@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — BASELINE.json metric: text-line-crops/sec (recognition), config 2.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Workload (BASELINE config 2 / SURVEY.md §8d): B = 256 synthetic 48x512 uint8 line crops per GPU -> 56x560,
 160 patches, 46-token prompt each; declared synthetic model SYN-REC (vision tower = reference defaults,
@@ -11,7 +11,8 @@ decoder 12 x 1280, GQA 16/4, vocab 65 792), bf16, greedy decode max_tokens = 128
   value : crops/s, whole job, inputs (fp32 tiles + index plan) already resident in HBM when the clock starts
   e2e   : crops/s through the public API (RecognitionRunner.run_preprocessed) from pinned HOST buffers,
           host->device copies of tiles/plan and device->host reads of tokens/scores/boxes inside the timed region
-  roofline     : dominant kernel = the tcgen05 GEMM in the HBM-bound decode step (see DESIGN.md §5)
+  roofline     : dominant kernel = the wgmma GEMM in the HBM-bound decode step (see DESIGN.md §5); peaks are the H100 SXM
+                 data sheet's (3.35 TB/s HBM3, 989 dense BF16 TFLOP/s), `gpu` gives the card and power limit measured on
   cpu_baseline : oracle port (fp32 PyTorch restatement of the reference modules) on this box's host cores,
                  bounded sample, rank 0 only
 
@@ -23,8 +24,12 @@ sb_rec_preprocess on the device vs the OpenCV thread pool; N = 1 only), `ocr_err
 
 Multi-GPU (torchrun, one rank per GPU): replicas over independent crop batches (weak scaling); one NCCL
 broadcast of the packed weights at init, one all_gather of the result tensors per step.
-`--impl reference` times the reference algorithm's CPU path (the oracle port: /root/reference is not on the GPU
-box and the reference is Python, so there is nothing to compile) on all host threads, same metric/config.
+`--impl reference` times the reference algorithm's CPU path (the oracle port; the reference is Python, so there is nothing
+to compile) on all host threads, same metric/config.
+
+`--dump-outputs DIR` writes what the timed recognition path computed in its last step — the prefill's and the 127 decode steps'
+tokens, scores, boxes and stop flags, i.e. what a caller of prefill + decode_steps receives — as DIR/<name>.npy (float32 or
+float64; integers are exact in float64).  Inputs and weights are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -69,11 +74,38 @@ def _peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"], "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 — upper bounds, not measured rates
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "src": "H100 SXM data sheet"}
+
+
+def gpu_info(index: int):
+    """Name, power limit and max SM clock of the card the numbers were measured on (they are part of the numbers)."""
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                            "-i", str(index)], capture_output=True, text=True, timeout=30)
+        name, power, clk = [c.strip() for c in r.stdout.strip().split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(clk)}
+    except Exception:      # noqa: BLE001
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
+
+
+def dump_outputs(out_dir: str, prefill_out: dict, hist: dict) -> dict:
+    """The last timed step's results as float32 / float64 .npy files (see the module docstring)."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    arrays = {f"prefill_{k}": prefill_out[k] for k in ("tok", "score", "bbox", "bbox_sig", "done", "next_ids")}
+    arrays.update({f"decode_{k}": v for k, v in hist.items()})
+    sizes = {}
+    for name, t in arrays.items():
+        a = t.detach().cpu()
+        a = a.double() if (a.dtype == torch.int64 or a.dtype == torch.float64) else a.float()
+        np.save(d / f"{name}.npy", a.numpy())
+        sizes[name] = list(a.shape)
+    return sizes
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -197,7 +229,7 @@ def run_reference_arm(args):
 # ------------------------------------------------------------------------------------------------ PyTorch-eager GPU arm
 def gpu_eager_baseline(dev, steps_rec=MAX_TOKENS):
     """The bar the kernels have to beat (SURVEY.md §8d, VERDICT r1 #6): the reference ALGORITHM in plain PyTorch eager on the
-    same B200 — cuBLAS GEMMs, F.scaled_dot_product_attention, DynamicCache-style concatenated KV (oracle/rec_oracle.py with
+    same GPU — cuBLAS GEMMs, F.scaled_dot_product_attention, DynamicCache-style concatenated KV (oracle/rec_oracle.py with
     FAST_ATTENTION, oracle/det_oracle.py), bf16 recognition / fp16 detection, same synthetic weights, same inputs, same work
     (256 crops x 128 tokens; 32 pages).  Secondary object, not the driver's reference arm."""
     from oracle import det_oracle as D
@@ -259,7 +291,7 @@ def _config(n_gpus):
             "model": "SYN-REC (declared synthetic: enc 8x1280/16h/I3420, dec 12x1280 GQA16/4 I3420, vocab 65792)",
             "global_batch": B_PER_GPU * n_gpus, "crops_per_gpu": B_PER_GPU, "max_tokens": MAX_TOKENS,
             "parallelism": f"replicas x{n_gpus} (independent crop batches)",
-            "l2": "no flush: per-step working set (0.96 GB weights + 0.5 GB KV + 1.2 GB activations) >> 126 MB L2"}
+            "l2": "no flush: per-step working set (0.96 GB weights + 0.5 GB KV + 1.2 GB activations) >> 50 MB L2"}
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
@@ -321,13 +353,8 @@ def decode_gemm_roofline(eng, peaks, reps=20):
     ms_step = e0.elapsed_time(e1) / reps
     n = len(calls)
     achieved = nbytes / n / (ms_step / n * 1e-3) / 1e9
-    traffic = None          # DRAM bytes per launch from the committed ncu capture of the same launches (profiles/)
-    tp = Path(__file__).resolve().parent / "profiles" / "decode_gemm_traffic.json"
-    if tp.exists():
-        traffic = json.loads(tp.read_text()).get("dram_bytes_per_launch")
     return {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-            "traffic": traffic, "traffic_src": "profiles/decode_gemm_traffic.json (ncu dram__bytes_read+write, per launch)",
-            "kernel": "gemm_tn_kernel / gemm_splitk_kernel (tcgen05), decode-step launches", "launches_per_decode_step": n,
+            "kernel": "gemm_tn_kernel / gemm_splitk_kernel (wgmma), decode-step launches", "launches_per_decode_step": n,
             "alg_bytes_per_launch": nbytes / n, "avg_launch_us": ms_step / n * 1e3, "gemm_ms_per_decode_step": ms_step,
             "gemm_tflops_in_decode": flops / (ms_step * 1e-3) / 1e12, "peak_src": peaks["src"]}, ms_step
 
@@ -593,6 +620,8 @@ def main():
     ap.add_argument("--no-layout", action="store_true", help="skip the layout / table_rec (config 4) secondary numbers")
     ap.add_argument("--no-pipeline", action="store_true", help="skip the ocr_text pipeline (config 5) secondary number")
     ap.add_argument("--no-ocr-error", action="store_true", help="skip the ocr_error (DistilBERT) secondary number")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's recognition outputs to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)
@@ -609,7 +638,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise _lib.SuryaB200Error("bench.py needs a B200 (no CPU fallback); use --impl reference for the CPU arm")
+        raise _lib.SuryaB200Error("bench.py needs a CUDA GPU (sm_90a; no CPU fallback); use --impl reference for the CPU arm")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -661,8 +690,11 @@ def main():
             "done": torch.empty((MAX_TOKENS - 1, B_PER_GPU), dtype=torch.uint8, device=dev)}
     from surya_b200 import shard
 
+    last = {}
+
     def resident_step():
         out = eng.prefill(tiles_dev, plan)
+        last["prefill"] = out
         ids_io.copy_(out["next_ids"])
         pos_io.copy_(lens)
         eng.decode_steps(ids_io, slot_t, pos_io, MAX_TOKENS - 1, hist=hist, max_pos=max_len)
@@ -703,6 +735,10 @@ def main():
     launches = _lib.launch_count() - l0
     ms_step = ms_total / args.steps
     value = B_PER_GPU * world * args.steps / (ms_total * 1e-3)
+    dumped = None
+    if args.dump_outputs and rank == 0:      # before the phase split below overwrites the histories
+        dumped = dump_outputs(args.dump_outputs, last["prefill"], hist)
+        log(f"outputs of the last timed step written to {args.dump_outputs}")
 
     # ---- phase split (CUDA events, rank-local, outside the headline region)
     def prefill_only():
@@ -805,9 +841,6 @@ def main():
             roof, gemm_ms = decode_gemm_roofline(eng, peaks)
             roof["share_of_step"] = gemm_ms * (MAX_TOKENS - 1) / ms_step          # of the whole step (prefill + 127 decode steps)
             roof["share_of_decode_step"] = gemm_ms / (ms_decode / (MAX_TOKENS - 1))
-            roof["share_note"] = ("ncu's launch list gives these launches 0.81 of one decode step's summed kernel time "
-                                  "(profiles/decode_gemm_traffic.json); in the graph ~0.10 ms of the 0.87 ms step is launch-to-launch "
-                                  "gap, which a sum of kernel durations does not contain")
         except Exception as e:      # noqa: BLE001
             roof = {"error": f"{type(e).__name__}: {e}"}
         # whole-step algorithmic bounds (SURVEY.md §8d) for context
@@ -836,6 +869,7 @@ def main():
             "data": "synthetic", "config": _config(world),
             "e2e": {"value": e2e_value, "unit": "crops/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": d2h_bytes,
                     "api": "surya_b200.recognition.RecognitionRunner.run_preprocessed (host tiles -> tokens/scores/boxes)"},
+            "gpu": gpu_info(local), "dumped_outputs": dumped,
             "gpu_launches": int(launches), "roofline": roof, "cpu_baseline": cpu, "gpu_eager_baseline": eager, "clocks": clocks,
             "phases_ms": {"prefill(vision+decoder)": ms_prefill, f"decode x{MAX_TOKENS - 1}": ms_decode,
                           "decode_step": ms_decode / (MAX_TOKENS - 1)},

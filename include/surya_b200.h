@@ -1,4 +1,4 @@
-/* surya_b200 — C ABI of libsurya_b200.so (sm_100a).
+/* surya_b200 — C ABI of libsurya_b200.so (sm_90a).
  *
  * The reference (VikParuchuri/surya v0.14.6) has no FFI: its seam is Python attribute access on
  * `predictor.model` (surya/common/predictor.py:20-29).  Every entry point below replaces one group of
@@ -304,7 +304,7 @@ int sb_det_text_front(int dtype, const void* logits, int n_labels, int B, int hs
 /* parity tap: copy workspace buffer `buf` (NHWC) into dst. */
 int sb_det_debug_copy(sb_det_engine* eng, int buf, void* dst, size_t bytes, void* stream);
 
-/* k x k dense convolution, NHWC, implicit GEMM on tcgen05 (op-level entry point used by the kernel tests). */
+/* k x k dense convolution, NHWC, implicit GEMM on wgmma (op-level entry point used by the kernel tests). */
 int sb_conv2d_nhwc(int dtype, const void* in, const void* weight, const float* bias, const void* residual, void* out,
                    int n_img, int H, int W, int Cin, int Cout, int ksize, int stride, int pad, int act, void* stream);
 int sb_dwconv_nhwc(int dtype, const void* in, const void* w, const float* bias, void* out, int B, int H, int W, int C,

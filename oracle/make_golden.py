@@ -1,8 +1,8 @@
-"""ORACLE TOOLING — generate golden vectors from the reference's own nn.Modules (run in the build container).
+"""ORACLE TOOLING — generate golden vectors from the reference's own nn.Modules and predictors.
 
-    python -m oracle.make_golden            # writes tests/golden/rec_*.pt
+    python -m oracle.make_golden [rec det layout table trace ocr_error pins]     # writes tests/golden/*.pt
 
-The reference (imported unmodified from /root/reference through oracle/ref_shim.py) is instantiated for a
+The reference (imported unmodified from $SURYA_REFERENCE through oracle/ref_shim.py) is instantiated for a
 declared config, loaded with surya_b200.synth's seeded weights, and driven exactly like
 RecognitionPredictor.prefill/decode drive it (surya/recognition/__init__.py:326-352, 398-409): one prefill
 with a fresh cache, then greedy decode steps feeding process_outputs' input_ids back.  Outputs are stored in
@@ -290,10 +290,161 @@ def make_ocr_error_golden():
         print(f"[golden] ocr_error_{kind}: logits {tuple(logits.shape)} labels={g['labels'].tolist()}")
 
 
+def det_heatmap_trials(seed: int, n: int, shape=(512, 640), boxes: int = 25, blur: float = 2.0, nested: bool = False):
+    """Seeded synthetic text heat maps (smooth blobs of text-line shape, 16-bit-valued like the engine's maps) for the
+    post-processing pins; the tests regenerate them with this same function."""
+    import cv2
+
+    rng = np.random.default_rng(seed)
+    H, W = shape
+    maps = []
+    for _ in range(n):
+        m = np.zeros((H, W), np.float32)
+        for _ in range(boxes):
+            if nested:
+                x, y = int(rng.integers(0, W - 60)), int(rng.integers(0, H - 30))
+                w, h = int(rng.integers(30, 220)), int(rng.integers(6, 30))
+            else:
+                x, y = int(rng.integers(0, 560)), int(rng.integers(0, 480))
+                w, h = int(rng.integers(30, 200)), int(rng.integers(6, 24))
+            m[y:y + h, x:x + w] = rng.uniform(0.3, 1.0)
+        if nested:
+            m[40:60, 100:300] = 0.9
+            m[44:56, 150:250] = 0.95                                   # a box contained in another one
+        maps.append(cv2.GaussianBlur(m, (0, 0), blur).astype(np.float16).astype(np.float32))
+    return maps, rng
+
+
+def ocr_error_texts():
+    rng = np.random.default_rng(0)
+    words = [f"w{i}" for i in range(300)]
+    return [" ".join(rng.choice(words, size=int(rng.integers(2, 30)))) for _ in range(8)]
+
+
+PREPROC_SIZES = ((48, 512), (40, 300), (300, 2000), (20, 60), (56, 560), (97, 1403))
+PREPROC_SAMPLE = 4096
+
+
+def make_reference_pins_golden():
+    """What the reference's own host code returns for the CPU pins in tests/ (processor, detection post-processing, predictors),
+    so that those tests run without the reference: tests/golden/reference_pins.pt."""
+    import hashlib
+
+    import torch.nn.functional as F2
+
+    from oracle import det_oracle as D
+    from oracle import ref_predictors as RP
+    from surya_b200.config import det_default, ocr_error_tiny
+    from surya_b200.synth import det_normalize, det_state_dict, ocr_error_state_dict
+
+    RP.install_predictors()
+    g = {"meta": {"reference": "VikParuchuri/surya@80e9a7e (v0.14.6), CPU", "torch": str(torch.__version__)}}
+
+    # SuryaOCRProcessor.scale_to_fit + _process_and_tile on seeded crops: grids, checksums and a seeded sample of the tiles
+    cfg = tiny_rec()
+    proc = RP.synthetic_ocr_processor(cfg)
+    rng = np.random.default_rng(11)
+    pre = []
+    for h, w in PREPROC_SIZES:
+        crop = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+        tiles, grid = proc._process_and_tile(proc.scale_to_fit(np.asarray(crop, dtype=np.float32), (1024, 256)))
+        flat = tiles.numpy().reshape(-1)
+        idx = np.random.default_rng(h * w).choice(flat.size, size=min(PREPROC_SAMPLE, flat.size), replace=False)
+        pre.append({"size": (h, w), "grid": tuple(int(v) for v in grid), "shape": tuple(tiles.shape),
+                    "idx": torch.from_numpy(idx), "sample": torch.from_numpy(flat[idx].copy()),
+                    "row_sums": torch.from_numpy(tiles.numpy().astype(np.float64).sum(1))})
+    g["preproc"] = pre
+
+    # surya.detection.heatmap: dynamic thresholds, detect_boxes, get_and_clean_boxes + expansion, slice_polys_from_image
+    from surya.detection.heatmap import detect_boxes, get_and_clean_boxes, get_dynamic_thresholds
+    from surya.input.processing import slice_polys_from_image
+    from surya.settings import settings
+
+    maps, _ = det_heatmap_trials(5, 3)
+    post = []
+    for m in maps:
+        tt, low = get_dynamic_thresholds(m, 0.6, 0.35)
+        boxes, conf = detect_boxes(m, 0.6, 0.35)
+        post.append({"tt": float(tt), "low": float(low), "boxes": [torch.from_numpy(np.asarray(b, np.float32)) for b in boxes],
+                     "conf": [float(c) for c in conf]})
+    g["det_postprocess"] = post
+    pipe = []
+    for trial in range(3):
+        m = det_heatmap_trials(9 * 1000 + trial, 1, boxes=20, blur=1.5, nested=True)[0][0]
+        H, W = m.shape
+        img_size = (W * 2, H * 2) if trial == 1 else (W, H)       # also exercise the rescale path
+        ref = get_and_clean_boxes(m, [W, H], img_size)
+        for box in ref:
+            if box.height < 3 * box.width:
+                box.expand(x_margin=0, y_margin=settings.DETECTOR_BOX_Y_EXPAND_MARGIN)
+                box.fit_to_bounds([0, 0, img_size[0], img_size[1]])
+        rec = {"img_size": img_size, "polygons": [[[float(v) for v in pt] for pt in r.polygon] for r in ref],
+               "conf": [float(r.confidence) for r in ref]}
+        if trial != 1:
+            page = np.random.default_rng(9 * 1000 + trial).integers(0, 256, size=(H, W, 3)).astype(np.float32)
+            slices = slice_polys_from_image(page, [[[int(v) for v in pt] for pt in r.polygon] for r in ref])
+            rec["slices"] = [(tuple(sl.shape), str(sl.dtype), hashlib.sha256(np.ascontiguousarray(sl).tobytes()).hexdigest())
+                             for sl in slices]
+        pipe.append(rec)
+    g["pipeline_host"] = pipe
+
+    # DetectionPredictor (BASELINE config 1) with the reference's own model on its own test page
+    from surya.detection import DetectionPredictor
+
+    from surya_b200 import dropin
+
+    dcfg = det_default()
+    dsd = det_state_dict(dcfg, seed=0)
+    ref_model = ref_shim.build_reference_det_model(dcfg, dsd)
+    dproc = RP.synthetic_det_processor(1024)
+    page = RP.conftest_page(1024)
+    Stock = type("StockDetectionPredictor", (DetectionPredictor,), {"model_loader_cls": dropin.loader_for(ref_model, dproc)})
+    stock = Stock(device="cpu", dtype=torch.float32)
+    stock.disable_tqdm = True
+    res = stock([page])[0]
+    x = torch.from_numpy(dproc(np.asarray(page, dtype=np.uint8))["pixel_values"][0])[None]
+    assert (x - det_normalize(np.asarray(page, dtype=np.uint8)[None])).abs().max() < 1e-5, "det_normalize no longer matches the processor"
+    with torch.inference_mode():
+        logits = ref_model(pixel_values=x).logits.float()
+    lidx = torch.from_numpy(np.random.default_rng(1).choice(logits.numel(), size=8192, replace=False))
+    g["det_config1"] = {"image_bbox": list(res.image_bbox), "polygons": [[[float(v) for v in pt] for pt in b.polygon] for b in res.bboxes],
+                        "logits_shape": tuple(logits.shape), "logit_idx": lidx, "logit_sample": logits.reshape(-1)[lidx].clone(),
+                        "page_checksum": x.double().sum()}
+    # the product's host chain (oracle heat maps -> thresholds -> boxes -> polygons) must reproduce those polygons
+    up = F2.interpolate(logits, size=[1024, 1024], mode="bilinear", align_corners=False)[0, 0].numpy()
+    tt, low, _ = D.dynamic_thresholds(up)
+    from surya_b200.detection import text_boxes_from_front
+    from surya_b200.pipeline import page_polygons
+
+    b, c = text_boxes_from_front(up, (up > low).astype(np.uint8), float(tt), float(low))
+    polys, _ = page_polygons(b, c, (1024, 1024), (1024, 1024))
+    assert [[[float(v) for v in pt] for pt in p] for p in polys] == g["det_config1"]["polygons"]
+
+    # OCRErrorPredictor over its own DistilBERT, batches of 3 with a ragged tail
+    from surya.ocr_error import OCRErrorPredictor
+
+    ecfg = ocr_error_tiny()
+    esd = ocr_error_state_dict(ecfg, seed=0)
+    sys.path.insert(0, str(ROOT / "tests"))
+    from test_ocr_error_cpu import _HashTokenizer
+
+    em = ref_shim.build_reference_ocr_error_model(ecfg, esd)
+    StockE = type("StockOCRErrorPredictor", (OCRErrorPredictor,), {"model_loader_cls": dropin.loader_for(em, _HashTokenizer(ecfg))})
+    se = StockE(device="cpu", dtype=torch.float32)
+    se.disable_tqdm = True
+    g["ocr_error_predictor"] = {"texts": ocr_error_texts(), "labels": list(se(ocr_error_texts(), batch_size=3).labels)}
+
+    torch.save(g, GOLDEN / "reference_pins.pt")
+    print(f"[golden] reference_pins: {len(pre)} processor crops, {len(post)} + {len(pipe)} heat maps, "
+          f"{len(g['det_config1']['polygons'])} config-1 boxes, labels {g['ocr_error_predictor']['labels']}")
+
+
 def main():
     GOLDEN.mkdir(parents=True, exist_ok=True)
     torch.set_num_threads(8)
-    which = set(sys.argv[1:]) or {"rec", "det", "layout", "table", "trace", "ocr_error"}
+    which = set(sys.argv[1:]) or {"rec", "det", "layout", "table", "trace", "ocr_error", "pins"}
+    if "pins" in which:
+        make_reference_pins_golden()
     if "layout" in which:
         make_layout_golden()
     if "table" in which:

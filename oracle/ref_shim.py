@@ -1,16 +1,18 @@
-"""ORACLE TOOLING (build container only) — import the *unmodified* reference from /root/reference.
+"""ORACLE TOOLING (golden generation only) — import the *unmodified* reference from the checkout named by $SURYA_REFERENCE
+(VikParuchuri/surya @ 80e9a7e).
 
 The reference pins transformers ^4.51 (pyproject.toml:15); this image has 5.5.  The few names that moved are
 patched *in transformers' namespace before import* (SURVEY.md §8c); no reference source is copied or edited.
-/root/reference does not exist on the GPU box: only oracle/make_golden.py (run here) uses this module.
+Only oracle/make_golden.py (and the helpers it calls) use this module; the tests read the fixtures it wrote.
 """
 from __future__ import annotations
 
+import os
 import sys
 import types
 from pathlib import Path
 
-REFERENCE = Path("/root/reference")
+REFERENCE = Path(os.environ.get("SURYA_REFERENCE", "") or "/nonexistent")
 
 
 def available() -> bool:
@@ -19,7 +21,7 @@ def available() -> bool:
 
 def install() -> None:
     if not available():
-        raise RuntimeError("/root/reference is not mounted: goldens can only be regenerated in the build container")
+        raise RuntimeError("set SURYA_REFERENCE to a checkout of VikParuchuri/surya@80e9a7e to regenerate the goldens")
     if str(REFERENCE) not in sys.path:
         sys.path.insert(0, str(REFERENCE))
     import torch

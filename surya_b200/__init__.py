@@ -1,4 +1,4 @@
-"""surya_b200 — Blackwell-native (sm_100a) engine for surya's batched model forward passes.
+"""surya_b200 — Hopper-native (sm_90a) engine for surya's batched model forward passes.
 
 Host side mirrors the reference's predictor/model call surface; every forward op is a hand-written CUDA
 kernel in libsurya_b200.so reached through the C ABI in include/surya_b200.h.  There is no CPU or

@@ -48,7 +48,7 @@ def load(require_cuda: bool = True) -> ctypes.CDLL:
         import torch
 
         if not torch.cuda.is_available():
-            raise SuryaB200Error("surya_b200 kernels need a CUDA device (sm_100a); none is visible")
+            raise SuryaB200Error("surya_b200 kernels need a CUDA device (sm_90a); none is visible")
     return _lib
 
 

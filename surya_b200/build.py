@@ -1,9 +1,8 @@
-"""In-tree build of libsurya_b200.so (sm_100a only).
+"""In-tree build of libsurya_b200.so (sm_90a only: the kernels use Hopper's wgmma, TMA and clusters).
 
-`nvcc -gencode arch=compute_100a,code=sm_100a` cross-compiles without a GPU, so the same function is
-used by `__graft_entry__.build()` in the CPU container and on a GPU box.  Objects are cached under
-`surya_b200/csrc/build/` (git-ignored) keyed by source + header mtimes; the shared library lands in
-`surya_b200/lib/` and travels to the GPU box with the repo snapshot.
+`nvcc -gencode arch=compute_90a,code=sm_90a` cross-compiles without a GPU, so the same function builds the
+library on a machine without one.  Objects are cached under `surya_b200/csrc/build/` (git-ignored) keyed by
+source + header mtimes; the shared library lands in `surya_b200/lib/` (git-ignored).
 """
 from __future__ import annotations
 
@@ -20,8 +19,9 @@ OBJDIR = CSRC / "build"
 LIBDIR = PKG / "lib"
 LIBNAME = "libsurya_b200.so"
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -34,7 +34,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and Path(cand).exists():
             return cand
-    raise RuntimeError("nvcc not found: surya_b200 needs the CUDA toolkit to build its sm_100a kernels")
+    raise RuntimeError("nvcc not found: surya_b200 needs the CUDA toolkit to build its sm_90a kernels")
 
 
 def _newest_header_mtime() -> float:
@@ -55,6 +55,11 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if not srcs:
         raise RuntimeError(f"no CUDA sources under {CSRC}")
     hdr_m = _newest_header_mtime()
+    # objects built with other flags (another architecture) are stale whatever their mtime
+    flags_file = OBJDIR / "nvcc_flags.txt"
+    flags = "\n".join(NVCC_FLAGS)
+    if not flags_file.exists() or flags_file.read_text() != flags:
+        force = True
     jobs = []
     objs = []
     for src in srcs:
@@ -80,9 +85,10 @@ def build(force: bool = False, verbose: bool = False) -> Path:
                 if verbose:
                     print(f"[surya_b200.build] compiled {name}", file=sys.stderr)
 
+    flags_file.write_text(flags)
     lib = lib_path()
     if jobs or not lib.exists() or any(o.stat().st_mtime > lib.stat().st_mtime for o in objs):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(lib), *map(str, objs)]
+        cmd = [nvcc, "-shared", *GENCODE, "-o", str(lib), *map(str, objs)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -6,7 +6,7 @@
 //                 (surya/common/surya/decoder/__init__.py:101-128, flash_attn_utils.py:106-154).
 //                 Tensor-core path: mma.sync m16n8k16 (fp32 accumulate), online softmax in fp32 registers,
 //                 P rounded to the storage type before the PV product (flash-attention semantics).
-//                 Attention is < 1 % of the recognition FLOPs (SURVEY.md §8a a10), the tcgen05 budget goes to the GEMMs.
+//                 Attention is < 1 % of the recognition FLOPs (SURVEY.md §8a a10), the tensor-core work is in the GEMMs.
 //  decode_attn  : q_len = 1 attention over the slot KV cache fused with RoPE(q,k) and the in-place cache append
 //                 (decoder/__init__.py:161-238 with DynamicCache.update -> no torch.cat, SURVEY.md §2.2 K10/K20).
 //                 HBM-bound: streams K and V once, CUDA-core FMA.
@@ -434,8 +434,7 @@ __global__ void __launch_bounds__(128) decode_attn_kernel(const DecodeKParams p)
 //           every thread requests the K row of "its" key into registers (one key per thread for up to 160 keys);
 //           the q / k / v slices of this row's fused qkv are requested.
 //   then    RoPE (q heads + new key) and the cache append, scores from the K registers, softmax, and P.V out of shared memory.
-// Round 1's kernel did these as three dependent phases (q/k row -> K -> V, the last one in up to three dependent batches):
-// 9 / 15 / 21 us at 46 / 110 / 173 cached tokens (profiles/r02_decode_parts.md).
+// The streaming kernel does these as three dependent phases (q/k row -> K -> V, the last one in up to three dependent batches).
 template <typename T, int HD, int G>
 __global__ void __launch_bounds__(160) decode_attn_v2_kernel(const DecodeKParams p) {
   constexpr int NT = 160, HALF = HD / 2, VPR = HD / 8;
@@ -631,9 +630,9 @@ static int launch_decode_v2(const DecodeAttnArgs& a, cudaStream_t st) {
   return launch_ok();
 }
 
-// OFF by default: measured 14 / 21 / 29 us against 9 / 15 / 21 us for the streaming kernel at 46 / 110 / 173 cached tokens
-// (B = 256, 4 kv heads): the 49 KB V tile allows 4 CTAs per SM instead of 10, the 1024 CTAs run in two lock-step waves and the
-// memory phase of a wave no longer overlaps anybody's arithmetic.  $SB_DECODE_ATTN_V2=1 enables it (tests cover both).
+// OFF by default: the 49 KB V tile allows far fewer CTAs per SM than the streaming kernel, so at B = 256 the CTAs run in
+// lock-step waves whose memory phase overlaps nobody's arithmetic (not re-measured on H100).  $SB_DECODE_ATTN_V2=1 enables it
+// (tests cover both).
 static bool decode_v2_enabled() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("SB_DECODE_ATTN_V2"); v = (e && e[0] == '1') ? 1 : 0; }

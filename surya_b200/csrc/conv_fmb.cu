@@ -3,14 +3,14 @@
 //
 // Stands in for FusedMBConv.forward (surya/detection/model/encoderdecoder.py:228-270) of the EfficientViT stages 0 and 1 and
 // replaces the op pair conv_igemm -> gemm of det_engine.cu.  At BASELINE config 3 the four blocks write and re-read
-// 2.1 + 1.0 + 1.0 + 0.5 GB of expanded activations per 32-page forward (profiles/r02_det_launch_summary.md).
+// 2.1 + 1.0 + 1.0 + 0.5 GB of expanded activations per 32-page forward.
 //
-// Back-to-back GEMM per 128-pixel tile (8 rows x 16 px):
+// Back-to-back GEMM per 128-pixel tile (8 rows x 16 px); two consumer warpgroups, each owning 64 of the tile's pixels end to end:
 //   for each chunk j of 128 mid channels:
-//     GEMM1  acc1[j & 1] (TMEM, 128 cols) = sum over 9 taps x Cin/BKC channel chunks of  A1 (tap box, TMA)  x  W1[j] (TMA)
-//     epi1   8 warps: acc1 + shift -> round -> Hardswish -> round -> 128B-swizzled A2 tile in shared memory (2 k-blocks of 64)
-//     GEMM2  acc2 (TMEM, Cout cols) += A2 x W2[:, chunk j] (TMA)          [issued after GEMM1(j+1): epi1(j) hides under it]
-//   epi2     4 warps: acc2 + shift (+ block input) -> round -> NHWC store
+//     GEMM1  acc1 (registers, 128 cols) = sum over 9 taps x Cin/BKC channel chunks of  A1 (tap box, TMA)  x  W1[j] (TMA)
+//     epi1   acc1 + shift -> round -> Hardswish -> round -> the warpgroup's 128B-swizzled A2 tile in shared memory (2 k-blocks)
+//     GEMM2  acc2 (registers, Cout cols) += A2 x W2[:, chunk j] (TMA)
+//   epi2     acc2 + shift (+ block input) -> round -> NHWC store
 // Rounding points are those of the two separate kernels (expand output in T after the shift, after Hardswish; project output
 // in T after the shift, after the residual add); the fp32 sum over the mid channels runs in the same k order as gemm_tn_kernel.
 #include "gemm.cuh"
@@ -38,45 +38,37 @@ struct FmbParams {
 };
 
 template <typename T, int BKC, int COUT, int STAGES, int NW2>
-__global__ void __launch_bounds__(512, 1)
+__global__ void __launch_bounds__(384, 1)
 fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_w1,
                  const __grid_constant__ CUtensorMap tma_w2, const FmbParams fp) {
-  constexpr int BM = 128, TW = 16, TH = 8, CH = 128;                 // mid-channel chunk
+  constexpr int TW = 16, TH = 8, CH = 128;                           // mid-channel chunk
   // Cin = 32 (BKC == 32): the nine tap tiles of a pixel tile stay RESIDENT for all mid-channel chunks (one 64-byte-row TMA box each per
   // tile instead of one per chunk) and W1 is streamed in [128 x 64] boxes that span a PAIR of taps (128-byte rows), which cuts the
-  // TMA line count per tile from 9216 to 3456 — the first version of this block was bound by the TMA engine, not by the tensor pipe.
+  // TMA line count per tile from 9216 to 3456.
   constexpr bool RES_A = (BKC == 32);
-  constexpr uint32_t A1_BYTES = BM * BKC * 2;
+  constexpr uint32_t A1_BYTES = 128 * BKC * 2;
   constexpr uint32_t W1_BYTES = RES_A ? CH * 64 * 2 : CH * BKC * 2;
   constexpr uint32_t S1_BYTES = RES_A ? W1_BYTES : A1_BYTES + W1_BYTES;
   constexpr uint32_t RESA_BYTES = RES_A ? 9 * A1_BYTES : 0;
-  constexpr uint32_t A2_KB_BYTES = BM * 64 * 2;                      // one 64-channel k-block of the A2 tile (16 KB)
-  constexpr uint32_t A2_BYTES = 2 * A2_KB_BYTES;                     // 128 mid channels
+  constexpr uint32_t A2_KB_BYTES = 64 * 64 * 2;                      // one 64-channel k-block of a warpgroup's A2 tile (8 KB)
+  constexpr uint32_t A2_WG_BYTES = 2 * A2_KB_BYTES;                  // 64 pixels x 128 mid channels
   constexpr uint32_t W2_KB_BYTES = COUT * 64 * 2, W2_BYTES = 2 * W2_KB_BYTES;
-  constexpr uint32_t TMEM_COLS = 512;                                // acc1: 2 x 128, acc2: COUT at column 256
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // array + offset keeps the shared address space (STS / LDS, not generic ST / LD)
   uint8_t* s_ra = smem;                                             // resident tap tiles (Cin = 32 only)
   uint8_t* s_1 = s_ra + RESA_BYTES;
   uint8_t* s_a2 = s_1 + STAGES * S1_BYTES;
-  uint8_t* s_w2 = s_a2 + 2 * A2_BYTES;
+  uint8_t* s_w2 = s_a2 + 2 * A2_WG_BYTES;
   float* s_b1 = reinterpret_cast<float*>(s_w2 + NW2 * W2_BYTES);
   float* s_b2 = s_b1 + fp.Cmid;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_b2 + COUT);
   uint64_t* s1_full = bars;
   uint64_t* s1_empty = s1_full + STAGES;
-  uint64_t* t1_full = s1_empty + STAGES;
-  uint64_t* t1_empty = t1_full + 2;
-  uint64_t* a2_full = t1_empty + 2;
-  uint64_t* a2_empty = a2_full + 2;
-  uint64_t* w2_full = a2_empty + 2;
+  uint64_t* w2_full = s1_empty + STAGES;
   uint64_t* w2_empty = w2_full + NW2;
-  uint64_t* t2_full = w2_empty + NW2;
-  uint64_t* t2_empty = t2_full + 1;
-  uint64_t* ra_full = t2_empty + 1;                                  // [9] resident tap tiles
+  uint64_t* ra_full = w2_empty + NW2;                                // [9] resident tap tiles
   uint64_t* ra_empty = ra_full + 9;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ra_empty + 9);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_img = fp.tiles_x * fp.tiles_y;
@@ -85,25 +77,16 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   const int cpb = fp.Cin / BKC;                                      // channel chunks per tap
   const int kb1 = 9 * cpb;                                           // GEMM1 k-blocks per mid chunk
 
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&tma_a); tma_prefetch_desc(&tma_w1); tma_prefetch_desc(&tma_w2); }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&s1_full[i], 1); mbar_init(&s1_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&t1_full[i], 1); mbar_init(&t1_empty[i], 8);
-      mbar_init(&a2_full[i], 8); mbar_init(&a2_empty[i], 1);
-    }
-    for (int i = 0; i < NW2; ++i) { mbar_init(&w2_full[i], 1); mbar_init(&w2_empty[i], 1); }
-    mbar_init(t2_full, 1); mbar_init(t2_empty, 4);
-    for (int i = 0; i < 9; ++i) { mbar_init(&ra_full[i], 1); mbar_init(&ra_empty[i], 1); }
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tma_a); tma_prefetch_desc(&tma_w1); tma_prefetch_desc(&tma_w2);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&s1_full[i], 1); mbar_init(&s1_empty[i], EPI_WARPS); }
+    for (int i = 0; i < NW2; ++i) { mbar_init(&w2_full[i], 1); mbar_init(&w2_empty[i], EPI_WARPS); }
+    for (int i = 0; i < 9; ++i) { mbar_init(&ra_full[i], 1); mbar_init(&ra_empty[i], EPI_WARPS); }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, TMEM_COLS);
   for (int i = threadIdx.x; i < fp.Cmid; i += blockDim.x) s_b1[i] = fp.bias1 ? fp.bias1[i] : 0.f;
   for (int i = threadIdx.x; i < COUT; i += blockDim.x) s_b2[i] = fp.bias2 ? fp.bias2[i] : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto coords = [&](int tile, int& img, int& oy0, int& ox0) {
     img = tile / tiles_per_img;
@@ -155,174 +138,118 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                 if (++s == STAGES) { s = 0; ph ^= 1; }
               }
           }
-          if (j >= 1) load_w2(j - 1);
+          load_w2(j);
         }
-        load_w2(nch - 1);
         raph ^= 1;
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc1 = umma_idesc_f16(TypeInfo<T>::umma_fmt, BM, CH);
-      constexpr uint32_t idesc2 = umma_idesc_f16(TypeInfo<T>::umma_fmt, BM, COUT);
-      int s = 0; uint32_t ph = 0; int wb = 0; uint32_t wph = 0; uint32_t raph = 0;
-      uint32_t t1ph[2] = {0, 0}, a2ph[2] = {0, 0}, t2ph = 0;
-      auto gemm2 = [&](int j) {
-        const int b = j & 1;
-        mbar_wait(&a2_full[b], a2ph[b]);
-        a2ph[b] ^= 1;
-        mbar_wait(&w2_full[wb], wph);
-        if (j == 0) { mbar_wait(t2_empty, t2ph ^ 1); }
-        tc_fence_after();
-        const uint32_t d2 = tmem_base + 256;
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-          const uint64_t da = umma_desc_k128(smem_u32(s_a2 + b * A2_BYTES + kk * A2_KB_BYTES));
-          const uint64_t db = umma_desc_k128(smem_u32(s_w2 + wb * W2_BYTES + kk * W2_KB_BYTES));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(d2, da + 2 * k, db + 2 * k, idesc2, (j | kk | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&a2_empty[b]);
-        umma_commit(&w2_empty[wb]);
-        if (++wb == NW2) { wb = 0; wph ^= 1; }
-      };
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        for (int j = 0; j < nch; ++j) {
-          const int b = j & 1;
-          mbar_wait(&t1_empty[b], t1ph[b] ^ 1);
-          t1ph[b] ^= 1;
-          tc_fence_after();
-          const uint32_t d1 = tmem_base + b * CH;
-          if constexpr (RES_A) {
-            for (int pr = 0; pr < 5; ++pr) {
-              mbar_wait(&s1_full[s], ph);
-              tc_fence_after();
-              const uint64_t dbp = umma_desc_k128(smem_u32(s_1 + s * S1_BYTES));     // [128 x 64]: taps 2pr (cols 0..31), 2pr+1 (32..63)
-              for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) {
-                if (j == 0) { mbar_wait(&ra_full[t], raph); tc_fence_after(); }
-                const uint64_t da = umma_desc_k64(smem_u32(s_ra + t * A1_BYTES));
-#pragma unroll
-                for (int k = 0; k < 2; ++k) umma_f16(d1, da + 2 * k, dbp + 4 * (t & 1) + 2 * k, idesc1, (t | k) != 0 ? 1u : 0u);
-                if (j == nch - 1) umma_commit(&ra_empty[t]);
-              }
-              umma_commit(&s1_empty[s]);
-              if (++s == STAGES) { s = 0; ph ^= 1; }
-            }
-          } else {
-          for (int kb = 0; kb < kb1; ++kb) {
-            mbar_wait(&s1_full[s], ph);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(s_1 + s * S1_BYTES);
-            const uint64_t da = (BKC == 64) ? umma_desc_k128(sa) : umma_desc_k64(sa);
-            const uint64_t db = (BKC == 64) ? umma_desc_k128(sa + A1_BYTES) : umma_desc_k64(sa + A1_BYTES);
-#pragma unroll
-            for (int k = 0; k < BKC / 16; ++k) umma_f16(d1, da + 2 * k, db + 2 * k, idesc1, (kb | k) != 0 ? 1u : 0u);
-            umma_commit(&s1_empty[s]);
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-          }
-          }
-          umma_commit(&t1_full[b]);
-          if (j >= 1) gemm2(j - 1);
-        }
-        gemm2(nch - 1);
-        umma_commit(t2_full);
-        t2ph ^= 1;
-        raph ^= 1;
-      }
-    }
-  } else if (warp >= 12) {
-    // ------------------------------------------------------------------ epilogue 2: project output
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    uint32_t t2ph = 0;
+  } else if (warp >= 4) {
+    // ------------------------------------------------------------------ consumer warpgroups: pixels [64 wg, 64 wg + 64) of the tile
+    const int wg = (warp - 4) >> 2, ww = warp & 3;
+    const int r0 = ww * 16 + (lane >> 2), c = (lane & 3) * 2;        // fragment rows r0, r0 + 8 (of the warpgroup), columns 8j + c
+    uint8_t* a2 = s_a2 + wg * A2_WG_BYTES;
+    int s = 0; uint32_t ph = 0; int wb = 0; uint32_t wph = 0; uint32_t raph = 0;
+    constexpr int NCH = 64;                                          // partial-sum width (register budget: d1 + d2 + part)
+    float d1[CH / 2], d2[COUT / 2], part[NCH / 2];
     T* out = reinterpret_cast<T*>(fp.out);
     const T* res = reinterpret_cast<const T*>(fp.residual);
+    auto release = [&](uint64_t* bar) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar);
+    };
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int img, oy0, ox0;
       coords(tile, img, oy0, ox0);
-      const int oy = oy0 + (row >> 4), ox = ox0 + (row & 15);
-      const bool ok = oy < fp.Ho && ox < fp.Wo;
-      const size_t pix = (static_cast<size_t>(img) * fp.Ho + (ok ? oy : 0)) * fp.Wo + (ok ? ox : 0);
-      mbar_wait(t2_full, t2ph);
-      t2ph ^= 1;
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + 256;
-#pragma unroll 1
-      for (int g = 0; g < COUT / 32; ++g) {
-        uint32_t v[32];
-        tmem_ld_32x32(tacc + g * 32, v);
-        tmem_ld_wait();
-        uint32_t o[16];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2)
-          o[j >> 1] = Pk<T>::pack(__uint_as_float(v[j]) + s_b2[g * 32 + j], __uint_as_float(v[j + 1]) + s_b2[g * 32 + j + 1]);
-        if (res && ok) {
-          const uint4* rp = reinterpret_cast<const uint4*>(res + pix * COUT + g * 32);
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const uint4 r4 = __ldg(rp + c);
-            const uint32_t rr[4] = {r4.x, r4.y, r4.z, r4.w};
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint32_t t = o[c * 4 + k];
-              o[c * 4 + k] = Pk<T>::pack(Pk<T>::lo(t) + Pk<T>::lo(rr[k]), Pk<T>::hi(t) + Pk<T>::hi(rr[k]));
-            }
-          }
-        }
-        if (ok) {
-          uint4* op = reinterpret_cast<uint4*>(out + pix * COUT + g * 32);
-#pragma unroll
-          for (int c = 0; c < 4; ++c) op[c] = make_uint4(o[c * 4], o[c * 4 + 1], o[c * 4 + 2], o[c * 4 + 3]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(t2_empty);
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue 1: expanded chunk -> A2 tile in shared memory
-    const int q = warp & 3, hh = (warp - 4) >> 2;          // lane quarter; 64-channel k-block of the chunk
-    const int row = q * 32 + lane;
-    uint32_t t1ph[2] = {0, 0}, a2ph[2] = {0, 0};
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       for (int j = 0; j < nch; ++j) {
-        const int b = j & 1;
-        mbar_wait(&t1_full[b], t1ph[b]);
-        t1ph[b] ^= 1;
-        tc_fence_after();
-        mbar_wait(&a2_empty[b], a2ph[b] ^ 1);              // GEMM2 of two chunks ago has read this A2 buffer
-        a2ph[b] ^= 1;
-        const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + b * CH + hh * 64;
-        uint8_t* dst = s_a2 + b * A2_BYTES + hh * A2_KB_BYTES + row * 128;
-        const float* bs = s_b1 + j * CH + hh * 64;
-#pragma unroll 1
-        for (int g = 0; g < 2; ++g) {
-          uint32_t v[32];
-          tmem_ld_32x32(tacc + g * 32, v);
-          tmem_ld_wait();
-          uint32_t o[16];
+        // GEMM1: expanded chunk j
+        // (per-k-block partial sums added in fp32, gemm_epilogue.cuh: one k-block = one tap here, as in conv_igemm with BKC = 32)
+        if constexpr (RES_A) {
 #pragma unroll
-          for (int jj = 0; jj < 32; jj += 2) {
-            const uint32_t t = Pk<T>::pack(__uint_as_float(v[jj]) + bs[g * 32 + jj], __uint_as_float(v[jj + 1]) + bs[g * 32 + jj + 1]);
-            o[jj >> 1] = Pk<T>::pack(act_ct<ACT_HARDSWISH>(Pk<T>::lo(t)), act_ct<ACT_HARDSWISH>(Pk<T>::hi(t)));
+          for (int i = 0; i < CH / 2; ++i) d1[i] = 0.f;
+          for (int pr = 0; pr < 5; ++pr) {
+            mbar_wait(&s1_full[s], ph);
+            if (j == 0)
+              for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) mbar_wait(&ra_full[t], raph);
+            const uint64_t dbp = wgmma_desc_k128(smem_u32(s_1 + s * S1_BYTES));     // [128 x 64]: taps 2pr (cols 0..31), 2pr+1 (32..63)
+            for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) {
+              const uint64_t da = wgmma_desc_k64(smem_u32(s_ra + t * A1_BYTES) + wg * 64 * 64);
+#pragma unroll
+              for (int cn = 0; cn < CH / NCH; ++cn) {
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 2; ++k)
+                  wgmma_m64k16<T, NCH>(part, da + 2 * k, dbp + ((cn * NCH * 128) >> 4) + 4 * (t & 1) + 2 * k, k != 0 ? 1u : 0u);
+                wgmma_commit();
+                wg_promote<NCH>(d1 + cn * (NCH / 2), part);
+              }
+            }
+            release(&s1_empty[s]);
+            if (j == nch - 1)
+              for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) release(&ra_empty[t]);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
           }
+        } else {
+          wg_mainloop<T, CH, BKC, NCH>(d1, s_1, S1_BYTES, A1_BYTES, STAGES, s1_full, s1_empty, s, ph, kb1, wg, lane,
+                                       [](const uint8_t*) {});
+        }
+        // epi1: + shift -> round -> Hardswish -> round -> A2 (row r, mid channel cc: k-block cc / 64, 16-byte chunk (cc % 64) / 8)
+        const float* bs = s_b1 + j * CH;
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const int ch = g * 4 + c;                       // 16-byte chunk inside the 128-byte row
-            *reinterpret_cast<uint4*>(dst + ((ch ^ (row & 7)) << 4)) = make_uint4(o[c * 4], o[c * 4 + 1], o[c * 4 + 2], o[c * 4 + 3]);
+        for (int jb = 0; jb < CH / 8; ++jb) {
+          const int cc = jb * 8 + c;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h;
+            const uint32_t t = Pk<T>::pack(d1[4 * jb + 2 * h] + bs[cc], d1[4 * jb + 2 * h + 1] + bs[cc + 1]);
+            const uint32_t o = Pk<T>::pack(act_ct<ACT_HARDSWISH>(Pk<T>::lo(t)), act_ct<ACT_HARDSWISH>(Pk<T>::hi(t)));
+            *reinterpret_cast<uint32_t*>(a2 + (cc >> 6) * A2_KB_BYTES + r * 128 + ((((cc & 63) >> 3) ^ (r & 7)) << 4) + (cc & 7) * 2) = o;
           }
         }
-        tc_fence_before();
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) { mbar_arrive(&t1_empty[b]); mbar_arrive(&a2_full[b]); }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> wgmma operand reads
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+        // GEMM2: acc2 += A2 x W2[:, chunk j], one 64-channel k-block at a time (the k-blocks of the unfused project GEMM)
+        mbar_wait(&w2_full[wb], wph);
+        if (j == 0) {
+#pragma unroll
+          for (int i = 0; i < COUT / 2; ++i) d2[i] = 0.f;
+        }
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          const uint64_t da = wgmma_desc_k128(smem_u32(a2 + kk * A2_KB_BYTES));
+          const uint64_t db = wgmma_desc_k128(smem_u32(s_w2 + wb * W2_BYTES + kk * W2_KB_BYTES));
+#pragma unroll
+          for (int cn = 0; cn < COUT / NCH; ++cn) {
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_m64k16<T, NCH>(part, da + 2 * k, db + ((cn * NCH * 128) >> 4) + 2 * k, k != 0 ? 1u : 0u);
+            wgmma_commit();
+            wg_promote<NCH>(d2 + cn * (NCH / 2), part);
+          }
+        }
+        release(&w2_empty[wb]);                                      // A2 and the W2 buffer are free again
+        if (++wb == NW2) { wb = 0; wph ^= 1; }
+      }
+      raph ^= 1;
+      // epi2: + shift (+ block input) -> round -> NHWC store
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = wg * 64 + r0 + 8 * h;                          // tile pixel (m / 16, m % 16)
+        const int oy = oy0 + (m >> 4), ox = ox0 + (m & 15);
+        if (oy >= fp.Ho || ox >= fp.Wo) continue;
+        const size_t pix = (static_cast<size_t>(img) * fp.Ho + oy) * fp.Wo + ox;
+#pragma unroll
+        for (int jb = 0; jb < COUT / 8; ++jb) {
+          const int cc = jb * 8 + c;
+          uint32_t o = Pk<T>::pack(d2[4 * jb + 2 * h] + s_b2[cc], d2[4 * jb + 2 * h + 1] + s_b2[cc + 1]);
+          if (res) {
+            const uint32_t rr = __ldg(reinterpret_cast<const unsigned int*>(res + pix * COUT + cc));
+            o = Pk<T>::pack(Pk<T>::lo(o) + Pk<T>::lo(rr), Pk<T>::hi(o) + Pk<T>::hi(rr));
+          }
+          *reinterpret_cast<uint32_t*>(out + pix * COUT + cc) = o;
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, TMEM_COLS); }
 }
 
 bool fmb_fused_ok(int Cin, int Cmid, int Cout, int ksize, int stride, int pad, int act1, int act2) {
@@ -330,9 +257,8 @@ bool fmb_fused_ok(int Cin, int Cmid, int Cout, int ksize, int stride, int pad, i
   if (en < 0) { const char* e = getenv("SB_FMB_FUSED"); en = e ? (e[0] - '0') : 1; }
   if (!en) return false;
   if (ksize != 3 || pad != 1 || (stride != 1 && stride != 2) || act1 != ACT_HARDSWISH || act2 != ACT_NONE) return false;
-  // Cin = 32 (stage 0, block 0) is instantiated and correct (bit-identical) but not faster than the two separate kernels: 1.38 vs
-  // 1.33 ms at B = 32 with per-chunk 64-byte tap boxes, and still no gain with resident tap tiles + tap-pair weight boxes (whole
-  // forward 18.52 vs 18.31 ms) -> opt-in with SB_FMB_FUSED=2
+  // Cin = 32 (stage 0, block 0) is instantiated and tested against the two separate kernels, but stays opt-in (SB_FMB_FUSED=2):
+  // its speed against them has not been measured on H100
   if (Cin == 32 && en < 2) return false;
   if (Cin != 32 && Cin != 64 && Cin != 128) return false;
   if (Cmid % 128 || Cmid < 128 || Cmid > 1024) return false;
@@ -343,7 +269,7 @@ template <typename T, int BKC, int COUT, int STAGES, int NW2>
 static int launch_fmb(int dtype, const void* in, const void* w1, const void* w2, const FmbParams& fp, cudaStream_t st) {
   constexpr bool RES_A = (BKC == 32);
   constexpr size_t S1 = RES_A ? static_cast<size_t>(128 * 64 * 2) : static_cast<size_t>(128 * BKC * 2) * 2;
-  const size_t SMEM = (RES_A ? 9 * 128 * 32 * 2 : 0) + STAGES * S1 + 2 * 32768 + NW2 * (COUT * 256) + (fp.Cmid + COUT) * 4 + 512 + 1024;
+  const size_t SMEM = (RES_A ? 9 * 128 * 32 * 2 : 0) + STAGES * S1 + 32768 + NW2 * (COUT * 256) + (fp.Cmid + COUT) * 4 + 512 + 1024;
   auto kern = fmb_fused_kernel<T, BKC, COUT, STAGES, NW2>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM) != cudaSuccess) {
     cudaGetLastError();
@@ -360,7 +286,7 @@ static int launch_fmb(int dtype, const void* in, const void* w1, const void* w2,
   if (rc) return rc;
   const int tiles = fp.n_img * fp.tiles_x * fp.tiles_y;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, 512, SMEM, st>>>(ma, m1, m2, fp);
+  kern<<<grid, 384, SMEM, st>>>(ma, m1, m2, fp);
   return launch_ok();
 }
 

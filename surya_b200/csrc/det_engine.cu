@@ -1,7 +1,7 @@
 // surya_b200 — detection engine: executes the EfficientViT-seg op program over NHWC workspaces.
 //
 // Stands in for EfficientViTForSemanticSegmentation.forward (surya/detection/model/encoderdecoder.py:725-753):
-// dense 3x3 convs -> conv_tcgen05.cu, 1x1 / grouped 1x1 convs -> gemm_tcgen05.cu, everything else -> det_ops.cu.
+// dense 3x3 convs -> conv_wgmma.cu, 1x1 / grouped 1x1 convs -> gemm_wgmma.cu, everything else -> det_ops.cu.
 #include "../../include/surya_b200.h"
 #include "ops.cuh"
 #include "sb_ptx.cuh"

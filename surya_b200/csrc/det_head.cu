@@ -3,19 +3,19 @@
 // (surya/detection/model/encoderdecoder.py:699-722) and replaces the op sequence upsample_cat -> gemm -> classifier of det_ops.cu.
 //
 // Why: at BASELINE config 3 (32 pages, 1024^2) the 512-channel map at 256^2 is 2.1 GB; the unfused path writes it twice and reads
-// it twice (8.6 GB of the ~24 GB a forward moves, 3.1 of 24.3 ms: profiles/r02_det_launch_summary.md).  Here it never exists:
+// it twice (8.6 GB of the ~24 GB a forward moves).  Here it never exists:
 //   * the A operand of the fuse GEMM (128 pixels x 512 channels per tile) is PRODUCED in shared memory: the three low-resolution
 //     branches by four builder warps (bilinear blend of the branch maps, which are L2 resident: 0.26 / 1 / 4 MB per page, with the
 //     same pinned arithmetic and the same rounding to the storage type as upsample_cat_kernel), the full-resolution branch by TMA;
-//     everything lands in the 128B-swizzled K-major layout tcgen05 reads;
-//   * the GEMM runs as two passes of N = 256 over the same A tile (TMEM: 2 x 256 fp32 columns, so the epilogue of one pass
-//     overlaps the MMAs of the other), weights streamed by TMA (32 KB per k-block and pass);
-//   * the epilogue adds the folded-BN shift, rounds to the storage type, applies ReLU and multiplies straight into the two
-//     classifier rows (FHFMA on the rounded 16-bit values, fp32 accumulation), so the fused map is never written either; the two
-//     column halves and the two passes meet in shared memory in a fixed order; sigmoid and the NCHW store finish the pixel.
+//     everything lands in the 128B-swizzled K-major layout wgmma reads;
+//   * two consumer warpgroups (64 pixels each) run the GEMM as eight passes of N = 64 over the same A tile, accumulators in
+//     registers (per-k-block partial sums added in fp32, like the unfused GEMM), weights streamed by TMA (8 KB per k-block and pass);
+//   * after each pass the epilogue adds the folded-BN shift, rounds to the storage type, applies ReLU and multiplies straight
+//     into the two classifier rows (fp32 accumulation of the rounded 16-bit values), so the fused map is never written either;
+//     the four lanes sharing a pixel meet through shuffles in a fixed order; sigmoid and the NCHW store finish the pixel.
 // Rounding points are those of the unfused kernels (branch value -> T, fuse output -> T, classifier logit -> T, sigmoid -> T);
-// only the fp32 summation order inside the 512-long classifier dot differs from classifier_kernel (lane-strided there, column
-// order here).
+// only the fp32 summation order inside the 512-long classifier dot differs from classifier_kernel (lane-strided there, strided by
+// the fragment layout here).
 #include "gemm.cuh"
 #include "gemm_epilogue.cuh"
 #include "ops.cuh"
@@ -48,49 +48,39 @@ struct HeadParams {
 template <typename T>
 __global__ void __launch_bounds__(512, 1)
 head_fused_kernel(const __grid_constant__ CUtensorMap tma_id, const __grid_constant__ CUtensorMap tma_w, const HeadParams hp) {
-  constexpr int BM = 128, TW = 16, TH = 8, BK = 64, BNH = 256;
-  constexpr uint32_t A_BYTES = BM * BK * 2;            // 16 KB per k-block
-  constexpr uint32_t W_BYTES = BNH * BK * 2;           // 32 KB per k-block and pass
-  constexpr int W_STAGES = 2;
-  constexpr uint32_t TMEM_COLS = 512;
+  constexpr int TW = 16, TH = 8, BK = 64, BNP = 64, PASSES = HEAD_N / BNP;
+  constexpr uint32_t A_BYTES = 128 * BK * 2;           // 16 KB per k-block
+  constexpr uint32_t W_BYTES = BNP * BK * 2;           // 8 KB per k-block and pass
+  constexpr int W_STAGES = 8;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // array + offset keeps the shared address space (STS / LDS, not generic ST / LD)
   uint8_t* s_a = smem;                                  // 8 x 16 KB
-  uint8_t* s_w = s_a + HEAD_KB * A_BYTES;               // 2 x 32 KB
+  uint8_t* s_w = s_a + HEAD_KB * A_BYTES;               // 8 x 8 KB
   float* s_bias = reinterpret_cast<float*>(s_w + W_STAGES * W_BYTES);      // [512]
   T* s_cls = reinterpret_cast<T*>(s_bias + HEAD_N);                          // [2][512]
-  float* s_part = reinterpret_cast<float*>(s_cls + 2 * HEAD_N);             // [2 halves][128 rows][2]
-  uint64_t* afull_bar = reinterpret_cast<uint64_t*>(s_part + 2 * BM * 2);
+  uint64_t* afull_bar = reinterpret_cast<uint64_t*>(s_cls + 2 * HEAD_N);
   uint64_t* aempty_bar = afull_bar + HEAD_KB;
   uint64_t* wfull_bar = aempty_bar + HEAD_KB;
   uint64_t* wempty_bar = wfull_bar + W_STAGES;
-  uint64_t* tfull_bar = wempty_bar + W_STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_img = hp.tiles_x * hp.tiles_y;
   const int num_tiles = hp.B * tiles_per_img;
   const int HW = hp.HO * hp.WO;
 
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&tma_id); tma_prefetch_desc(&tma_w); }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < HEAD_KB; ++i) { mbar_init(&afull_bar[i], hp.src[i] ? 4 : 1); mbar_init(&aempty_bar[i], 1); }
-    for (int i = 0; i < W_STAGES; ++i) { mbar_init(&wfull_bar[i], 1); mbar_init(&wempty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], EPI_WARPS); }
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tma_id); tma_prefetch_desc(&tma_w);
+    for (int i = 0; i < HEAD_KB; ++i) { mbar_init(&afull_bar[i], hp.src[i] ? 4 : 1); mbar_init(&aempty_bar[i], EPI_WARPS); }
+    for (int i = 0; i < W_STAGES; ++i) { mbar_init(&wfull_bar[i], 1); mbar_init(&wempty_bar[i], EPI_WARPS); }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, TMEM_COLS);
   for (int i = threadIdx.x; i < HEAD_N; i += blockDim.x) {
     s_bias[i] = hp.fuse_bias[i];
     s_cls[i] = reinterpret_cast<const T*>(hp.cls_w)[i];
     s_cls[HEAD_N + i] = reinterpret_cast<const T*>(hp.cls_w)[HEAD_N + i];
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto coords = [&](int tile, int& img, int& oy0, int& ox0) {
     img = tile / tiles_per_img;
@@ -100,7 +90,7 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tma_id, const __grid_const
   };
 
   if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer: weights (both passes) + identity-branch A blocks
+    // ------------------------------------------------------------------ TMA producer: weights (every pass) + identity-branch A blocks
     if (lane == 0) {
       int ws_ = 0; uint32_t wph = 0; uint32_t aph = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -113,42 +103,14 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tma_id, const __grid_const
           tma_load_4d(s_a + kb * A_BYTES, &tma_id, &afull_bar[kb], hp.tma_c0[kb], ox0, oy0, img);
         }
         aph ^= 1;
-        for (int h = 0; h < 2; ++h) {
+        for (int h = 0; h < PASSES; ++h) {
           for (int kb = 0; kb < HEAD_KB; ++kb) {
             mbar_wait(&wempty_bar[ws_], wph ^ 1);
             mbar_expect_tx(&wfull_bar[ws_], W_BYTES);
-            tma_load_2d(s_w + ws_ * W_BYTES, &tma_w, &wfull_bar[ws_], kb * BK, h * BNH);
+            tma_load_2d(s_w + ws_ * W_BYTES, &tma_w, &wfull_bar[ws_], kb * BK, h * BNP);
             if (++ws_ == W_STAGES) { ws_ = 0; wph ^= 1; }
           }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(TypeInfo<T>::umma_fmt, BM, BNH);
-      int ws_ = 0; uint32_t wph = 0; uint32_t aph = 0; uint32_t tph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        for (int h = 0; h < 2; ++h) {
-          mbar_wait(&tempty_bar[h], tph ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + h * BNH;
-          for (int kb = 0; kb < HEAD_KB; ++kb) {
-            if (h == 0) mbar_wait(&afull_bar[kb], aph);
-            mbar_wait(&wfull_bar[ws_], wph);
-            tc_fence_after();
-            const uint64_t da = umma_desc_k128(smem_u32(s_a + kb * A_BYTES));
-            const uint64_t db = umma_desc_k128(smem_u32(s_w + ws_ * W_BYTES));
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_commit(&wempty_bar[ws_]);
-            if (h == 1) umma_commit(&aempty_bar[kb]);
-            if (++ws_ == W_STAGES) { ws_ = 0; wph ^= 1; }
-          }
-          umma_commit(&tfull_bar[h]);
-        }
-        aph ^= 1;
-        tph ^= 1;
       }
     }
   } else if (warp >= 12) {
@@ -169,7 +131,7 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tma_id, const __grid_const
         uint8_t* dst = s_a + kb * A_BYTES;
         // two batches of four pixel rows: 16 independent 16-byte loads in flight per thread before the first blend.  The x / y
         // weights of an integer up-sampling ratio (2, 4, 8) are multiples of 1/16, exact in the 16-bit storage type, so the blend
-        // runs on FHFMA without converting the loaded values: p = lx*b + hx*a, q = lx*d + hx*c (both exact products + one
+        // runs on fma16 (exact 16-bit products) of the loaded values: p = lx*b + hx*a, q = lx*d + hx*c (both exact products + one
         // rounding each, identical to the fp32 expression), then hy*p + ly*q in fp32.
 #pragma unroll 1
         for (int half = 0; half < 2; ++half) {
@@ -218,68 +180,81 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tma_id, const __grid_const
       aph ^= 1;
     }
   } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue: + shift, round, ReLU, classifier dot, sigmoid
-    const int q = warp & 3, hh = (warp - 4) >> 2;           // lane quarter; 128-column half of the pass
-    const int row = q * 32 + lane;
-    uint32_t tph = 0;
+    // ------------------------------------------------------------------ consumers: MMA passes, + shift, round, ReLU, classifier dot, sigmoid
+    const int wg = (warp - 4) >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c = (lane & 3) * 2;   // fragment rows r0, r0 + 8; columns 8j + c
+    int ws_ = 0; uint32_t wph = 0; uint32_t aph = 0;
     const unsigned short* wc0 = reinterpret_cast<const unsigned short*>(s_cls);
     const unsigned short* wc1 = wc0 + HEAD_N;
+    float d[BNP / 2], part[BNP / 2];
+    auto release = [&](uint64_t* bar) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar);
+    };
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int img, oy0, ox0;
       coords(tile, img, oy0, ox0);
-      float d0 = 0.f, d1 = 0.f;
-      for (int h = 0; h < 2; ++h) {
-        mbar_wait(&tfull_bar[h], tph);
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + h * BNH + hh * 128;
-        const int col_base = h * BNH + hh * 128;
-#pragma unroll 1
-        for (int g = 0; g < 4; ++g) {
-          uint32_t v[32];
-          tmem_ld_32x32(tacc + g * 32, v);
-          tmem_ld_wait();
-          const int cb = col_base + g * 32;
+      float dot[2][2] = {{0.f, 0.f}, {0.f, 0.f}};     // [row r0 / r0 + 8][classifier output]
+      for (int h = 0; h < PASSES; ++h) {
 #pragma unroll
-          for (int j = 0; j < 32; j += 2) {
-            const float x0 = fmaxf(__uint_as_float(v[j]) + s_bias[cb + j], 0.f);
-            const float x1 = fmaxf(__uint_as_float(v[j + 1]) + s_bias[cb + j + 1], 0.f);
+        for (int i = 0; i < BNP / 2; ++i) d[i] = 0.f;
+        for (int kb = 0; kb < HEAD_KB; ++kb) {
+          if (h == 0) mbar_wait(&afull_bar[kb], aph);
+          mbar_wait(&wfull_bar[ws_], wph);
+          const uint64_t da = wgmma_desc_k128(smem_u32(s_a + kb * A_BYTES) + wg * 64 * 128);
+          const uint64_t db = wgmma_desc_k128(smem_u32(s_w + ws_ * W_BYTES));
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) wgmma_m64k16<T, BNP>(part, da + 2 * k, db + 2 * k, k != 0 ? 1u : 0u);
+          wgmma_commit();
+          wg_promote<BNP>(d, part);
+          release(&wempty_bar[ws_]);
+          if (h == PASSES - 1) release(&aempty_bar[kb]);
+          if (++ws_ == W_STAGES) { ws_ = 0; wph ^= 1; }
+        }
+#pragma unroll
+        for (int jb = 0; jb < BNP / 8; ++jb) {
+          const int cb = h * BNP + jb * 8 + c;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const float x0 = fmaxf(d[4 * jb + 2 * hh] + s_bias[cb], 0.f);
+            const float x1 = fmaxf(d[4 * jb + 2 * hh + 1] + s_bias[cb + 1], 0.f);
             const uint32_t pk = Pk<T>::pack(x0, x1);        // rounded to T: what the unfused path stores
             const unsigned short lo = static_cast<unsigned short>(pk & 0xffffu), hi = static_cast<unsigned short>(pk >> 16);
-            d0 = fma16<T>(lo, wc0[cb + j], d0);
-            d1 = fma16<T>(lo, wc1[cb + j], d1);
-            d0 = fma16<T>(hi, wc0[cb + j + 1], d0);
-            d1 = fma16<T>(hi, wc1[cb + j + 1], d1);
+            dot[hh][0] = fma16<T>(lo, wc0[cb], dot[hh][0]);
+            dot[hh][1] = fma16<T>(lo, wc1[cb], dot[hh][1]);
+            dot[hh][0] = fma16<T>(hi, wc0[cb + 1], dot[hh][0]);
+            dot[hh][1] = fma16<T>(hi, wc1[cb + 1], dot[hh][1]);
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[h]);
       }
-      tph ^= 1;
-      // the two column halves meet in shared memory (fixed order: half 0 + half 1)
-      asm volatile("bar.sync 1, 256;" ::: "memory");       // previous tile's partials have been consumed
-      s_part[(hh * BM + row) * 2] = d0;
-      s_part[(hh * BM + row) * 2 + 1] = d1;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (hh == 0) {
-        const int oy = oy0 + (row >> 4), ox = ox0 + (row & 15);
-        if (oy < hp.HO && ox < hp.WO) {
-          const T* cb_ = reinterpret_cast<const T*>(hp.cls_b);
-          T* out = reinterpret_cast<T*>(hp.out);
+      aph ^= 1;
+      // the four lanes holding a pixel's columns meet in a fixed order
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int o = 0; o < 2; ++o) {
+          dot[hh][o] += __shfl_xor_sync(0xffffffffu, dot[hh][o], 1);
+          dot[hh][o] += __shfl_xor_sync(0xffffffffu, dot[hh][o], 2);
+        }
+      if ((lane & 3) == 0) {
+        const T* cb_ = reinterpret_cast<const T*>(hp.cls_b);
+        T* out = reinterpret_cast<T*>(hp.out);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = r0 + 8 * hh;
+          const int oy = oy0 + (row >> 4), ox = ox0 + (row & 15);
+          if (oy >= hp.HO || ox >= hp.WO) continue;
           const size_t pix = static_cast<size_t>(oy) * hp.WO + ox;
 #pragma unroll
           for (int o = 0; o < 2; ++o) {
-            const float acc = s_part[row * 2 + o] + s_part[(BM + row) * 2 + o];
-            const float v = rnd<T>(acc + to_f<T>(cb_[o]));
+            const float v = rnd<T>(dot[hh][o] + to_f<T>(cb_[o]));
             out[(static_cast<size_t>(img) * 2 + o) * HW + pix] = from_f<T>(1.f / (1.f + expf(-v)));
           }
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, TMEM_COLS); }
 }
 
 bool det_head_fused_ok(int n_src, int CS, int n_out, int cin, int cout, const int* hs, const int* ws, int HO, int WO) {
@@ -299,7 +274,7 @@ bool det_head_fused_ok(int n_src, int CS, int n_out, int cin, int cout, const in
 
 template <typename T>
 static int launch_head(const HeadParams& hp, const CUtensorMap& mid, const CUtensorMap& mw, cudaStream_t st) {
-  constexpr size_t SMEM = 8 * 16384 + 2 * 32768 + 512 * 4 + 2 * 512 * 2 + 2 * 128 * 2 * 4 + 512 + 1024;
+  constexpr size_t SMEM = 8 * 16384 + 8 * 8192 + 512 * 4 + 2 * 512 * 2 + 512 + 1024;
   auto kern = head_fused_kernel<T>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -341,7 +316,7 @@ int det_head_fused(int dtype, const void* const* srcs, const int* hs, const int*
   CUtensorMap mid, mw;
   int rc = make_tma_nhwc(&mid, dtype, ident, B, HO, WO, CS, 64, 16, 8, 1, 128);
   if (rc) return rc;
-  rc = make_tma_2d(&mw, dtype, fuse_w, 512, 512, 512, 256);
+  rc = make_tma_2d(&mw, dtype, fuse_w, 512, 512, 512, 64);
   if (rc) return rc;
   return dtype == DT_BF16 ? launch_head<__nv_bfloat16>(hp, mid, mw, st) : launch_head<__half>(hp, mid, mw, st);
 }

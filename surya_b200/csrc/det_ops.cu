@@ -101,10 +101,9 @@ int det_stem_conv(int dtype, const void* in, int in_f32, const float* w, const f
 // CTA = 32 output columns x 8 channel vectors (64 channels = one 128 B line per pixel); every thread owns 8 channels of one
 // output column and walks TY output rows with the k x k weights in registers, so each input row it touches is loaded once per
 // column instead of once per tap row (L1 absorbs the overlap between neighbouring columns).  fp32 accumulation in tap order
-// (r, s) — the same order as a direct per-pixel loop.  Round 2: the multiply-adds are FHFMA (16-bit operands, fp32 accumulate,
-// sb_ptx.cuh fma16): 322 -> 285 us for the 64x64x1024 stage-2 layer at B = 32, 202 -> 159 us for the 5x5.  A shared-memory-tiled,
-// double-buffered persistent variant (cp.async halo tiles, 2 CTAs/SM) was measured at 356 us and dropped (git history:
-// "shared-memory tiled ... depthwise 3x3"): the kernel is not bound by the L1 re-fetch of neighbouring columns.
+// (r, s) — the same order as a direct per-pixel loop; the multiply-adds take the 16-bit operands as loaded (sb_ptx.cuh fma16).
+// A shared-memory-tiled, double-buffered persistent variant (cp.async halo tiles, 2 CTAs/SM) was slower and dropped (git
+// history: "shared-memory tiled ... depthwise 3x3"): the kernel is not bound by the L1 re-fetch of neighbouring columns.
 template <typename T, int KS, int STRIDE, int TY>
 __global__ void __launch_bounds__(256, 2) dwconv_kernel(const T* __restrict__ in, const T* __restrict__ w,
                                                         const float* __restrict__ bias, T* __restrict__ out, int H, int W, int C,
@@ -227,8 +226,7 @@ int det_dwconv(int dtype, const void* in, const void* w, const float* bias, void
 // qkv_a / qkv_b: token-major [B*HW, 3*heads*DIM] (plain qkv and aggregated qkv); head h of scale s reads channels
 // [h*3*DIM, (h+1)*3*DIM) = (q | k | v).  out: [B*HW, 2*heads*DIM], channel = (s*heads + h)*DIM + d.
 // One CTA per (image, scale*heads + h).  fp32 throughout; rounded to T once at the end (reference: .float() ... .to(dtype)).
-// Round 2 re-tiling (profiles/r02_det_kernels_ncu.md: the first version was shared-memory bound, L1/TEX 88 %, 2.5 FMA per LDS in
-// phase 1 and one broadcast LDS.128 per 4 FMA in phase 2):
+// Tiling (a first version was shared-memory bound: 2.5 FMA per LDS in phase 1 and one broadcast LDS.128 per 4 FMA in phase 2):
 //   phase 1  kv[i][j] = sum_t relu(k[t][i]) * [v[t] | 1][j]: thread = (2 rows i, 8 columns j, one quarter of each token tile):
 //            3 shared loads per 18 FMA; the four token-quarters meet in shared memory in a fixed order;
 //   phase 2  out[t] = relu(q[t]) kv: thread = (4 tokens, 8 columns): 2 LDS.128 + 1 LDS.32 per 36 FMA; every thread also carries

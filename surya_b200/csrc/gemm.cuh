@@ -1,4 +1,4 @@
-// surya_b200 — tcgen05 GEMM interface (host side). See gemm_tcgen05.cu.
+// surya_b200 — wgmma GEMM interface (host side). See gemm_wgmma.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -47,7 +47,7 @@ struct GemmArgs {
   int am_ld = 0;
   int store_c = 1;
 };
-// M <= 16 rows: mma.sync kernel without the tcgen05 set-up costs (gemm_skinny.cu); gemm_launch routes to it when it applies.
+// M <= 16 rows: mma.sync kernel without the wgmma pipeline set-up costs (gemm_skinny.cu); gemm_launch routes to it when it applies.
 bool gemm_skinny_ok(const GemmArgs& a);
 int gemm_skinny_launch(const GemmArgs& a, cudaStream_t stream);
 // Several dependent skinny GEMMs in one persistent launch with grid-wide barriers between them (gemm_chain.cu); `bar` = 3

@@ -2,19 +2,18 @@
 //
 //   for phase in phases:   C_p[M, Nout_p] = epilogue_p(A_p[M, K_p] @ W_p[N_p, K_p]^T)        A_{p+1} may be C_p
 //
-// Why (profiles/r02_decode_parts.md): inside the decode graph a 256-row GEMM costs 8.7 - 13.9 us of which ~6 us is not data
-// movement — launch, block scheduling behind the previous kernel's 200 KB CTAs, barrier / TMEM / descriptor set-up, pipeline
-// ramp, drain and the completion -> dependent-launch hand-over.  A decoder layer is a chain  o_proj -> gate_up -> down ->
+// Why: inside the decode graph a 256-row GEMM spends a large share of its time on things other than data movement — launch,
+// block scheduling behind the previous kernel's 200 KB CTAs, barrier / descriptor set-up, pipeline ramp, drain and the
+// completion -> dependent-launch hand-over.  A decoder layer is a chain  o_proj -> gate_up -> down ->
 // next layer's qkv  where each GEMM needs the complete rows of its predecessor, so the kernels cannot be fused tile-wise; they
-// CAN share one launch: all 148 CTAs stay resident, set up once, and cross a grid-wide barrier (one global counter, release /
+// CAN share one launch: one CTA per SM stays resident, set up once, and cross a grid-wide barrier (one global counter, release /
 // acquire) between phases.  Numerics are those of gemm_tn_kernel with the same tile width (same k order, same epilogue).
 //
-// Layout of a CTA (384 threads) is gemm_tn_kernel's: warp 0 = TMA producer, warp 1 = tcgen05.mma issuer, warp 2 = TMEM
-// allocator, warps 4-11 = epilogue (+ the in-kernel sum of squares of the folded RMSNorm).  Differences:
-//   * the tile width BN is a per-phase RUNTIME value (32 / 64 / 96 / 128): one 6-stage ring of 32 KB slots (16 KB of A + up to
-//     16 KB of W) serves every phase, the instruction descriptor is built per phase, accumulators sit 128 columns apart;
-//   * the "stage free" barriers always expect the MMA commit plus the 8 epilogue warps (they walk the k-blocks of every phase;
-//     they only read the stage when the phase folds an RMSNorm), so no barrier is re-initialised between phases;
+// Layout of a CTA (384 threads) is gemm_tn_kernel's: warp 0 = TMA producer, warps 4-11 = two consumer warpgroups (wgmma, the
+// in-kernel sum of squares of the folded RMSNorm, epilogue).  Differences:
+//   * the tile width BN is a per-phase RUNTIME value (32 / 64 / 96 / 128, dispatched to a compile-time main loop): one 4-stage
+//     ring of 32 KB slots (16 KB of A + up to 16 KB of W) serves every phase, the accumulator tile has 128-column rows;
+//   * the ring's barriers keep their phase across phases of the chain, so no barrier is re-initialised;
 //   * grid barrier: bar[0] counts arrivals (monotonic inside a launch), bar[1] counts exits; the last CTA to leave resets both.
 //     Every CTA is resident by construction (grid <= SM count, 1 CTA / SM); a spin that exceeds 2 s raises bar[2] and moves on
 //     so that a scheduling surprise produces a loud error instead of a hung GPU.
@@ -27,11 +26,10 @@ namespace sb {
 int make_tma_2d(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_rows);
 
 constexpr int CH_MAX_PHASES = 4;
-constexpr int CH_STAGES = 6;
+constexpr int CH_STAGES = 4;
 constexpr int CH_BN_MAX = 128;
 constexpr uint32_t CH_A_BYTES = 128 * 64 * 2;
 constexpr uint32_t CH_SLOT_BYTES = CH_A_BYTES + CH_BN_MAX * 64 * 2;          // 32 KB
-constexpr uint32_t CH_TMEM_COLS = 2 * CH_BN_MAX;
 
 struct ChainPhase {
   int M, N, K, bn;
@@ -47,7 +45,7 @@ struct ChainParams {
   unsigned int* bar;       // [0] arrivals, [1] exits, [2] timeout flag
   int group_m;
   unsigned long long* dbg; // optional timeline of CTA 0 (globaltimer ns): [8*phase + {0 start, 1 first tile data landed,
-                           // 2 last MMA issued, 3 accumulator ready, 4 epilogue done, 5 barrier passed}]
+                           // 3 accumulator ready, 4 epilogue done, 5 barrier passed}]
 };
 struct ChainMaps { CUtensorMap a[CH_MAX_PHASES]; CUtensorMap b[CH_MAX_PHASES]; };
 
@@ -102,10 +100,8 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // array + offset keeps the shared address space (STS / LDS, not generic ST / LD)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + CH_STAGES * CH_SLOT_BYTES);
   uint64_t* empty_bar = full_bar + CH_STAGES;
-  uint64_t* tfull_bar = empty_bar + CH_STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  uint8_t* epi_smem = smem + CH_STAGES * CH_SLOT_BYTES + 256;
+  float* acc_s = reinterpret_cast<float*>(smem + CH_STAGES * CH_SLOT_BYTES + 256);      // [128][CH_BN_MAX] accumulator tile
+  uint8_t* epi_smem = reinterpret_cast<uint8_t*>(acc_s) + acc_smem_bytes<CH_BN_MAX>();
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -116,31 +112,18 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
       tma_prefetch_desc(&maps.a[i]);
       tma_prefetch_desc(&maps.b[i]);
     }
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < CH_STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1 + EPI_WARPS);        // MMA commit + the 8 epilogue warps, in every phase
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], EPI_WARPS);
+      mbar_init(&empty_bar[i], EPI_WARPS);
     }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, CH_TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // pipeline state, carried across phases by each role
-  int s = 0;            // producer / MMA: ring slot
-  uint32_t ph = 0;      //                 and its phase bit
-  int as = 0;           // MMA / epilogue: accumulator buffer
-  uint32_t aph = 0;
-  int es = 0;           // epilogue: ring slot seen by the per-k-block pass
-  uint32_t eph = 0;
+  int s = 0;            // ring slot
+  uint32_t ph = 0;      // and its phase bit
+  float d[CH_BN_MAX / 2];
 
   auto stamp = [&](int slot) {
     if (p.dbg && blockIdx.x == 0) p.dbg[slot] = globaltimer_ns();
@@ -189,41 +172,17 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
           }
         }
       }
-    } else if (warp == 1) {
-      // ---------------------------------------------------------------- MMA issuer
-      if (lane == 0) {
-        const uint32_t idesc = umma_idesc_f16(TypeInfo<T>::umma_fmt, BM, static_cast<uint32_t>(bn));
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-          mbar_wait(&tempty_bar[as], aph ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + as * CH_BN_MAX;
-          for (int kb = 0; kb < k_blocks; ++kb) {
-            mbar_wait(&full_bar[s], ph);
-            tc_fence_after();
-            if (kb == 0 && tile == static_cast<int>(blockIdx.x)) stamp(8 * pi + 1);
-            const uint32_t sa = smem_u32(smem + s * CH_SLOT_BYTES);
-            const uint64_t da = umma_desc_k128(sa);
-            const uint64_t db = umma_desc_k128(sa + CH_A_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_commit(&empty_bar[s]);
-            if (++s == CH_STAGES) { s = 0; ph ^= 1; }
-          }
-          umma_commit(&tfull_bar[as]);
-          if (tile == static_cast<int>(blockIdx.x)) stamp(8 * pi + 2);
-          as ^= 1;
-          if (as == 0) aph ^= 1;
-        }
-      }
     } else if (warp >= 4) {
-      // ---------------------------------------------------------------- epilogue warps
+      // ---------------------------------------------------------------- consumer warpgroups: MMA + epilogue
       if (pi == 0) pdl_wait();
+      const int wg = (warp - 4) >> 2;
       const int q = warp & 3;
-      const int half = (warp - 4) >> 2;
+      const int half = wg;
       const int epi_tid = threadIdx.x - 128;
       uint8_t* stage = epi_smem + (warp - 4) * EPI_STAGE_BYTES;
       float* sbias = reinterpret_cast<float*>(epi_smem + EPI_WARPS * EPI_STAGE_BYTES);
       float* srs = sbias + CH_BN_MAX;
+      const AccRow acc(acc_s, q * 32 + lane, CH_BN_MAX);
       GemmKParams g{};
       g.M = P.M; g.N = P.N; g.K = P.K; g.C = P.C; g.ldc = P.ldc; g.bias = P.bias; g.residual = P.residual; g.ldr = P.ldr;
       g.act = P.act; g.swiglu = P.swiglu;
@@ -233,49 +192,46 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
         asm volatile("bar.sync 1, 256;" ::: "memory");
         epilogue_stage_bias_rt(g, sbias, epi_tid, nb * bn, bn);
         asm volatile("bar.sync 1, 256;" ::: "memory");
-        {
-          // walk the k-blocks: release every stage (the barrier expects us) and, when the phase folds an RMSNorm, take the
-          // rows' sum of squares from the A tile on the way
-          float acc = 0.f;
-          for (int kb = 0; kb < k_blocks; ++kb) {
-            mbar_wait(&full_bar[es], eph);
-            if (P.ssq_inline) acc = ssq_stage<T>(smem + es * CH_SLOT_BYTES, epi_tid, acc);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[es]);
-            if (++es == CH_STAGES) { es = 0; eph ^= 1; }
-          }
-          if (P.ssq_inline) {
-            const float tot = acc + __shfl_xor_sync(0xffffffffu, acc, 1);
-            if ((epi_tid & 1) == 0) srs[epi_tid >> 1] = rsqrtf(tot * P.ssq_inv_k + P.ssq_eps);
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-          }
+        // main loop; when the phase folds an RMSNorm, the rows' sum of squares is taken from the A tiles on the way
+        float ssq = 0.f;
+        const bool first = tile == static_cast<int>(blockIdx.x);
+        bool landed = false;
+        auto on_stage = [&](const uint8_t* slot) {
+          if (first && !landed && epi_tid == 0) stamp(8 * pi + 1);
+          landed = true;
+          if (P.ssq_inline) ssq = ssq_stage<T>(slot, epi_tid, ssq);
+        };
+        switch (bn) {
+          case 32: wg_mainloop<T, 32, BK>(d, smem, CH_SLOT_BYTES, CH_A_BYTES, CH_STAGES, full_bar, empty_bar, s, ph, k_blocks, wg, lane, on_stage); break;
+          case 64: wg_mainloop<T, 64, BK>(d, smem, CH_SLOT_BYTES, CH_A_BYTES, CH_STAGES, full_bar, empty_bar, s, ph, k_blocks, wg, lane, on_stage); break;
+          case 96: wg_mainloop<T, 96, BK>(d, smem, CH_SLOT_BYTES, CH_A_BYTES, CH_STAGES, full_bar, empty_bar, s, ph, k_blocks, wg, lane, on_stage); break;
+          default: wg_mainloop<T, 128, BK>(d, smem, CH_SLOT_BYTES, CH_A_BYTES, CH_STAGES, full_bar, empty_bar, s, ph, k_blocks, wg, lane, on_stage); break;
         }
-        mbar_wait(&tfull_bar[as], aph);
-        tc_fence_after();
-        if (warp == 4 && lane == 0 && tile == static_cast<int>(blockIdx.x)) stamp(8 * pi + 3);
-        const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * CH_BN_MAX;
+        if (P.ssq_inline) {
+          const float tot = ssq + __shfl_xor_sync(0xffffffffu, ssq, 1);
+          if ((epi_tid & 1) == 0) srs[epi_tid >> 1] = rsqrtf(tot * P.ssq_inv_k + P.ssq_eps);
+        }
+        if (epi_tid == 0 && first) stamp(8 * pi + 3);
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // the accumulator tile is free
+        float* dst = acc_s + wg * 64 * CH_BN_MAX;
+        switch (bn) {
+          case 32: wg_acc_store<4>(d, 0, dst, CH_BN_MAX, warp & 3, lane); break;
+          case 64: wg_acc_store<8>(d, 0, dst, CH_BN_MAX, warp & 3, lane); break;
+          case 96: wg_acc_store<12>(d, 0, dst, CH_BN_MAX, warp & 3, lane); break;
+          default: wg_acc_store<16>(d, 0, dst, CH_BN_MAX, warp & 3, lane); break;
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
         const int row0 = mb * BM + q * 32;
         const float rs = P.ssq_inline ? srs[q * 32 + lane] : 1.0f;
-        epilogue_tile_rt<T>(tacc, g, stage, sbias, lane, half, [&](int r) { return row0 + r < P.M ? row0 + r : -1; }, nb * bn, rs,
+        epilogue_tile_rt<T>(acc, g, stage, sbias, lane, half, [&](int r) { return row0 + r < P.M ? row0 + r : -1; }, nb * bn, rs,
                             bn / 32);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[as]);
-        if (warp == 4 && lane == 0 && tile == static_cast<int>(blockIdx.x)) stamp(8 * pi + 4);
-        as ^= 1;
-        if (as == 0) aph ^= 1;
+        if (epi_tid == 0 && first) stamp(8 * pi + 4);
       }
     }
     if (pi + 1 < p.n_phases) chain_grid_sync(p.bar, static_cast<unsigned int>(pi + 1) * gridDim.x);
     if (threadIdx.x == 0) stamp(8 * pi + 5);
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, CH_TMEM_COLS);
-  }
   if (threadIdx.x == 0 && p.n_phases > 1) {
     __threadfence();
     const unsigned int old = atomicAdd(&p.bar[1], 1u);
@@ -303,7 +259,8 @@ int gemm_chain_bn(int M, int N, int swiglu) {
 
 template <typename T>
 static int chain_launch_typed(const GemmArgs* ph, int n, unsigned int* bar, cudaStream_t stream) {
-  constexpr size_t SMEM = CH_STAGES * CH_SLOT_BYTES + 1024 + 256 + EPI_WARPS * EPI_STAGE_BYTES + CH_BN_MAX * 4 + EPI_ROWSCALE_BYTES;
+  constexpr size_t SMEM = CH_STAGES * CH_SLOT_BYTES + 1024 + 256 + acc_smem_bytes<CH_BN_MAX>() + epi_smem_bytes<CH_BN_MAX>();
+  static_assert(SMEM <= 227 * 1024, "gemm_chain does not fit in shared memory");
   auto kern = gemm_chain_kernel<T>;
   static bool attr_set = false;
   if (!attr_set) {

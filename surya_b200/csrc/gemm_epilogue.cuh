@@ -1,5 +1,8 @@
-// surya_b200 — epilogue shared by the tcgen05 GEMM and implicit-GEMM convolution kernels.
-// One call handles the 32 accumulator columns a thread just pulled from TMEM for its output row.
+// surya_b200 — main loop and epilogue shared by the wgmma GEMM and implicit-GEMM convolution kernels.
+//
+// A 128-row tile is computed by two consumer warpgroups (warps 4-11 of the CTA), each issuing m64 wgmma over its 64 rows
+// from the TMA ring; their register accumulators are then staged in a shared-memory tile (AccTile) from which the epilogue
+// reads one output row per thread, 32 columns at a time.
 #pragma once
 #include "gemm.cuh"
 #include "sb_ptx.cuh"
@@ -132,17 +135,105 @@ __device__ __noinline__ void epilogue_chunk(const uint32_t (&v)[32], const GemmK
 }
 
 
-// ---------------------------------------------------------------------------------------------------------------
-// Tile epilogue (8 warps): TMEM -> registers -> packed 16-bit math -> swizzled per-warp staging -> coalesced global.
+// ------------------------------------------------------------------------------------------------- accumulator tile
+// fp32 [128 rows][ld] in shared memory, ld a multiple of 32; 16-byte chunks XOR-swizzled by (row & 7), so that the fragment
+// stores and the row-per-lane 16-byte reads both spread over the banks without padding.
+__device__ __forceinline__ int acc_off(int row, int col, int ld) {
+  return row * ld + ((((col >> 2) ^ (row & 7))) << 2) + (col & 3);
+}
+constexpr int ACC_MAX_COLS = 128;   // accumulator columns staged per epilogue pass (wider tiles take two passes)
+template <int BN> constexpr int acc_cols() { return BN < ACC_MAX_COLS ? BN : ACC_MAX_COLS; }
+template <int BN> constexpr int acc_smem_bytes() { return 128 * acc_cols<BN>() * 4; }
+
+// This thread's output row of the staged accumulator tile.
+struct AccRow {
+  const float* row;
+  int sw;
+  __device__ __forceinline__ AccRow(const float* tile, int r, int ld) : row(tile + r * ld), sw(r & 7) {}
+  // 32 consecutive fp32 accumulators starting at column col0 (a multiple of 32)
+  __device__ __forceinline__ void load32(int col0, uint32_t (&v)[32]) const {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float4 x = *reinterpret_cast<const float4*>(row + ((((col0 >> 2) + i) ^ sw) << 2));
+      v[4 * i] = __float_as_uint(x.x); v[4 * i + 1] = __float_as_uint(x.y);
+      v[4 * i + 2] = __float_as_uint(x.z); v[4 * i + 3] = __float_as_uint(x.w);
+    }
+  }
+};
+
+// n8 blocks [j0, j0 + NB) of this warpgroup's m64 fragment -> columns [0, 8 NB) of rows [0, 64) of `dst` (the warpgroup's
+// first row in the accumulator tile; a multiple of 8, so the swizzle of a local row equals that of the tile row).
+template <int NB>
+__device__ __forceinline__ void wg_acc_store(const float* d, int j0, float* dst, int ld, int wg_warp, int lane) {
+  const int r0 = wg_warp * 16 + (lane >> 2), c = (lane & 3) * 2;
+#pragma unroll
+  for (int jj = 0; jj < NB; ++jj) {
+    const int j = j0 + jj;
+    *reinterpret_cast<float2*>(dst + acc_off(r0, jj * 8 + c, ld)) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(dst + acc_off(r0 + 8, jj * 8 + c, ld)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+
+// One consumer warpgroup's share of a 128 x BN tile: k_blocks slots of the TMA ring (slot = A [128 x BK] then W [BN x BK],
+// K-major, swizzled rows of BK * 2 bytes), BK / 16 MMAs per slot on A rows [64 wg, 64 wg + 64).  on_stage(slot) runs while the
+// slot's first MMAs execute (the folded RMSNorm reads the A rows there); the slot is released (one arrival per warp on
+// empty_bar) once its MMAs have completed.
 //
-// History (profiles/r01_gemm_prefill_ncu.md, tools/gemm_timeline.py): the first epilogue (epilogue_chunk above, kept as
-// the generic fallback) was instruction-fetch bound and took 30-40 us per 128x256 tile; staging + compile-time
-// activation brought it to 12.6 us, still longer than the 8.4 us main loop.  This version
-//   * runs on 8 warps (two per TMEM lane quarter, alternating 64/32-column groups) so each SM sub-partition has two
-//     epilogue warps to interleave;
-//   * stages the tile's bias slice in shared memory once, before the accumulator is ready (overlaps the main loop);
+// Accumulation: the tensor core adds its products into the accumulator with truncation, so over a long K the error of a
+// single accumulator chain grows with K and is biased.  Each slot's MMAs therefore run into a fresh partial (NCH columns at a
+// time, NCH <= BN) that is then added to d in fp32 with round-to-nearest: d = ((0 + p_0) + p_1) + ...  Every kernel that
+// must agree bit for bit with another (fused vs unfused, chain vs separate launches, any tile width) sums this way, per
+// k-block of the same K order.
+template <typename T, int BN, int BK, int NCH = (BN < ACC_MAX_COLS ? BN : ACC_MAX_COLS), typename StageFn>
+__device__ __forceinline__ void wg_mainloop(float* d, const uint8_t* ring, uint32_t slot_bytes, uint32_t a_bytes, int stages,
+                                            uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& ph, int k_blocks,
+                                            int wg, int lane, StageFn on_stage) {
+  static_assert(BN % NCH == 0, "column chunks must tile the accumulator");
+  float t[NCH / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+  for (int kb = 0; kb < k_blocks; ++kb) {
+    mbar_wait(&full_bar[s], ph);
+    const uint8_t* slot = ring + s * slot_bytes;
+    const uint32_t sa = smem_u32(slot);
+    const uint64_t da = wgmma_desc_kmajor<BK * 2>(sa + wg * 64 * BK * 2);
+    const uint64_t db = wgmma_desc_kmajor<BK * 2>(sa + a_bytes);
+#pragma unroll
+    for (int c = 0; c < BN / NCH; ++c) {
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        wgmma_m64k16<T, NCH>(t, da + 2 * k, db + ((c * NCH * BK * 2) >> 4) + 2 * k, k != 0 ? 1u : 0u);
+      wgmma_commit();
+      if (c == 0) on_stage(slot);
+      wgmma_wait<0>();
+      acc_fence<NCH / 2>(t);
+#pragma unroll
+      for (int i = 0; i < NCH / 2; ++i) d[c * (NCH / 2) + i] += t[i];
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
+    if (++s == stages) { s = 0; ph ^= 1; }
+  }
+}
+
+// The same per-k-block accumulation for kernels that issue their own MMAs: partial t (N columns) is complete; d += t.
+template <int N>
+__device__ __forceinline__ void wg_promote(float* d, float* t) {
+  wgmma_wait<0>();
+  acc_fence<N / 2>(t);
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] += t[i];
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Tile epilogue (8 warps): accumulator tile -> registers -> packed 16-bit math -> swizzled per-warp staging -> coalesced global.
+//
+// epilogue_chunk above is the generic fallback; this version
+//   * runs on 8 warps (two per 32-row quarter of the tile, alternating 32-column groups);
+//   * stages the tile's bias slice in shared memory once, before the main loop;
 //   * keeps the per-element instruction count minimal: packed cvt (cvt.rn.bf16x2.f32 / f16x2), one rounding per eager
-//     op boundary, residual fetched with coalesced 16-byte loads issued before the TMEM load they overlap with;
+//     op boundary, residual fetched with coalesced 16-byte loads (cp.async, one group ahead);
 //   * moves every global byte as part of a 64/128-byte row segment (XOR-swizzled staging, conflict-free).
 // Requires ldc % 8 == 0, ldr % 8 == 0, N % 8 == 0 (N % 16 == 0 and act == silu with SwiGLU), 16-bit output.
 constexpr int EPI_WARPS = 8;
@@ -201,14 +292,14 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, boo
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-// One warp, one tile.  taddr: TMEM address (lane quarter, first accumulator column of the tile); row_fn(r): global output
+// One warp, one tile.  acc: this lane's row of the accumulator tile (column 0 = weight row n_col0); row_fn(r): global output
 // row of the warp's r-th row or -1; n_col0: first weight row (accumulator column) of the tile; half: 0/1 = which of the two
-// warps sharing this lane quarter; sbias: the tile's bias slice (BN floats, already staged, zeros when absent).
+// warps sharing this row quarter; sbias: the tile's bias slice (already staged, zeros when absent).
 // stage: 4 KB per warp = residual sub-tile (cp.async, prefetched one group ahead) + output sub-tile, both swizzled.
 template <typename T, int ACT, bool SWIGLU, typename RowFn>
-__device__ __forceinline__ void epilogue_tile_ct(uint32_t taddr, const GemmKParams& p, uint8_t* stage, const float* sbias,
+__device__ __forceinline__ void epilogue_tile_ct(const AccRow& acc, const GemmKParams& p, uint8_t* stage, const float* sbias,
                                                  int lane, int half, RowFn row_fn, int n_col0, float rs, const int NG) {
-  constexpr int GW = 32;                            // accumulator columns per group (one tcgen05.ld .x32); NG groups per tile
+  constexpr int GW = 32;                            // accumulator columns per group; NG groups per tile
   constexpr int GWO = SWIGLU ? GW / 2 : GW;         // output columns per group
   constexpr int CPR = GWO / 8;                      // 16-byte chunks per staged row
   constexpr int ITERS = CPR;                        // 32 rows x CPR chunks / 32 lanes
@@ -242,8 +333,7 @@ __device__ __forceinline__ void epilogue_tile_ct(uint32_t taddr, const GemmKPara
     uint32_t o[GWO / 2];                            // this lane's packed output row segment
     {
       uint32_t v[32];
-      tmem_ld_32x32(taddr + g * GW, v);
-      tmem_ld_wait();
+      acc.load32(g * GW, v);
       const float* bs = sbias + g * GW;
 #pragma unroll
       for (int j = 0; j < 32; j += 4) {
@@ -298,7 +388,7 @@ __device__ __forceinline__ void epilogue_tile_ct(uint32_t taddr, const GemmKPara
 }
 
 // Online (max, first argmax, sum exp(x - max)) over the tile's columns for this lane's row; logits are rounded to the storage
-// type first (the reference takes argmax / softmax of the 16-bit lm_head output cast to fp32).  The two warps of a lane
+// type first (the reference takes argmax / softmax of the 16-bit lm_head output cast to fp32).  The two warps of a row
 // quarter cover alternating 32-column groups; their partials meet in shared memory (`xch` = base of the epilogue staging blocks) and warp half 0 writes
 // the (row, n-tile) partial.  Columns beyond N are skipped.
 struct AmPartial { float m; int i; float s; };
@@ -315,7 +405,7 @@ __device__ __forceinline__ void am_combine(AmPartial& a, const AmPartial& b) {
 }
 
 template <typename T, int BN>
-__device__ __forceinline__ void epilogue_tile_argmax(uint32_t taddr, const GemmKParams& p, uint8_t* xch, const float* sbias,
+__device__ __forceinline__ void epilogue_tile_argmax(const AccRow& acc, const GemmKParams& p, uint8_t* xch, const float* sbias,
                                                      int lane, int half, int q, int row, int n_col0, int nb, float rs) {
   constexpr int GW = 32, NG = BN / GW;
   AmPartial a{-INFINITY, 0x7fffffff, 0.f};
@@ -324,8 +414,7 @@ __device__ __forceinline__ void epilogue_tile_argmax(uint32_t taddr, const GemmK
     const int acol0 = n_col0 + g * GW;
     if (acol0 >= p.N) break;
     uint32_t v[32];
-    tmem_ld_32x32(taddr + g * GW, v);
-    tmem_ld_wait();
+    acc.load32(g * GW, v);
     const float* bs = sbias + g * GW;
     float x[32];
     float cm = -INFINITY;
@@ -400,27 +489,27 @@ __device__ __forceinline__ void epilogue_stage_bias_rt(const GemmKParams& p, flo
 
 // Runtime -> compile-time dispatch on (act, swiglu); once per tile, outside every loop.  ng = 32-column groups in the tile.
 template <typename T, typename RowFn>
-__device__ __forceinline__ void epilogue_tile_rt(uint32_t taddr, const GemmKParams& p, uint8_t* stage, const float* sbias,
+__device__ __forceinline__ void epilogue_tile_rt(const AccRow& acc, const GemmKParams& p, uint8_t* stage, const float* sbias,
                                                  int lane, int half, RowFn row_fn, int n_col0, float rs, int ng) {
   if (p.swiglu) {   // SwiGLU (Qwen2 MLPs) or GeGLU (ADETR MLP, gelu_pytorch_tanh)
-    if (p.act == ACT_SILU) epilogue_tile_ct<T, ACT_SILU, true>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng);
-    else epilogue_tile_ct<T, ACT_GELU_TANH, true>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng);
+    if (p.act == ACT_SILU) epilogue_tile_ct<T, ACT_SILU, true>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng);
+    else epilogue_tile_ct<T, ACT_GELU_TANH, true>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng);
     return;
   }
   switch (p.act) {
-    case ACT_NONE: epilogue_tile_ct<T, ACT_NONE, false>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
-    case ACT_GELU_ERF: epilogue_tile_ct<T, ACT_GELU_ERF, false>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
-    case ACT_HARDSWISH: epilogue_tile_ct<T, ACT_HARDSWISH, false>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
-    case ACT_RELU: epilogue_tile_ct<T, ACT_RELU, false>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
-    case ACT_SILU: epilogue_tile_ct<T, ACT_SILU, false>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
-    default: epilogue_tile_ct<T, ACT_GELU_TANH, false>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
+    case ACT_NONE: epilogue_tile_ct<T, ACT_NONE, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
+    case ACT_GELU_ERF: epilogue_tile_ct<T, ACT_GELU_ERF, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
+    case ACT_HARDSWISH: epilogue_tile_ct<T, ACT_HARDSWISH, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
+    case ACT_RELU: epilogue_tile_ct<T, ACT_RELU, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
+    case ACT_SILU: epilogue_tile_ct<T, ACT_SILU, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
+    default: epilogue_tile_ct<T, ACT_GELU_TANH, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
   }
 }
 
 template <typename T, int BN, typename RowFn>
-__device__ __forceinline__ void epilogue_tile_v2(uint32_t taddr, const GemmKParams& p, uint8_t* stage, const float* sbias,
+__device__ __forceinline__ void epilogue_tile_v2(const AccRow& acc, const GemmKParams& p, uint8_t* stage, const float* sbias,
                                                  int lane, int half, RowFn row_fn, int n_col0, float rs = 1.0f) {
-  epilogue_tile_rt<T>(taddr, p, stage, sbias, lane, half, row_fn, n_col0, rs, BN / 32);
+  epilogue_tile_rt<T>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, BN / 32);
 }
 
 }  // namespace sb

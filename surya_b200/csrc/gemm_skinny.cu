@@ -2,9 +2,8 @@
 //
 //   C[M, Nout] = epilogue(A[M, K] @ W[N, K]^T), same contract and rounding points as gemm_tn_kernel.
 //
-// Why: at 16 rows the tcgen05 kernel's fixed costs (TMEM allocation, mbarrier / tensor-map set-up, a 128-row MMA tile that is
-// 7/8 padding, 9.6 us per launch inside the decode graph, profiles/r01c_layout_launch_summary.md) dwarf the work: a decode step
-// of the layout decoder is 48 such GEMMs.  This kernel is the light-weight path: weights stream straight from HBM into
+// Why: at 16 rows the wgmma kernel's fixed costs (mbarrier / tensor-map set-up, a 128-row MMA tile that is 7/8 padding)
+// dwarf the work: a decode step of the layout decoder is 48 such GEMMs.  This kernel is the light-weight path: weights stream straight from HBM into
 // registers (16 B per lane, fully coalesced), the 16 activation rows come from L2, and the products run on mma.sync
 // m16n8k16 — M = 16 is exactly one MMA tile, so no tensor-core lane is padding.
 //   * CTA = 8 warps = one group of 8 output columns; the warps split K eight ways and meet in shared memory in warp order

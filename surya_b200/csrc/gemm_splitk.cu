@@ -1,6 +1,6 @@
-// surya_b200 — split-K tcgen05 GEMM for skinny problems (decode steps: M <= 256 rows against a large weight matrix).
+// surya_b200 — split-K wgmma GEMM for skinny problems (decode steps: M <= 256 rows against a large weight matrix).
 //
-//   C[M, Nout] = epilogue(A[M, K] @ W[N, K]^T), same contract as gemm_tn_kernel (gemm_tcgen05.cu).
+//   C[M, Nout] = epilogue(A[M, K] @ W[N, K]^T), same contract as gemm_tn_kernel (gemm_wgmma.cu).
 //
 // Why: with M = 256 the plain kernel needs many small N tiles to occupy the SMs, and every CTA re-reads a whole 128-row slab
 // of A (80 % of its bytes at BN = 32) from L2 — the launch is bound by L2 throughput on activation re-reads
@@ -10,8 +10,9 @@
 // (st.shared::cluster), one cluster barrier, then j sums the PK partials in rank order (deterministic) and runs the usual
 // epilogue (bias -> round -> act -> round -> (+residual | SwiGLU product) -> round) on its slice.
 //
-// Roles per CTA (192 threads): warp 0 = TMA producer (weight tiles requested before griddepcontrol.wait), warp 1 = TMEM
-// allocator + single-thread tcgen05.mma issuer, warps 2-5 = epilogue (one per TMEM lane quarter).
+// Roles per CTA (384 threads): warp 0 = TMA producer (weight tiles requested before griddepcontrol.wait), warps 4-11 = two
+// consumer warpgroups (wgmma on rows [0, 64) / [64, 128), then the scatter of their fragments); warps 4-7 run the final epilogue
+// (one per 32-row quarter).
 #include "gemm.cuh"
 #include "gemm_epilogue.cuh"
 #include "sb_ptx.cuh"
@@ -30,8 +31,8 @@ __device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t ra
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
   return r;
 }
-__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void st_cluster_f2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.aligned;" ::: "memory"); }
@@ -39,7 +40,7 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-constexpr int SK_THREADS = 192;
+constexpr int SK_THREADS = 384;
 constexpr int SK_MAX_PK = 8;
 
 // first 8-column unit owned by rank j when n_units units are dealt to pk ranks
@@ -51,17 +52,13 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
                    int pk, int rstride, int STAGES) {
   constexpr int BM = 128, BK = 64;
   constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr uint32_t TMEM_COLS = BN <= 32 ? 32 : BN <= 64 ? 64 : BN <= 128 ? 128 : 256;
   constexpr int N_UNITS = BN / 8;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // array + offset keeps the shared address space (STS / LDS, not generic ST / LD)
-  // STAGES (<= 8) is a launch parameter: as many pipeline stages as fit beside the receive buffer — the main loop needs
-  // ~150 KB in flight per SM to run at the SM's L2 read-port rate (profiles/r01_gemm_decode_microbench.md)
+  // STAGES (<= 8) is a launch parameter: as many pipeline stages as fit beside the receive buffer
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + 8;
-  uint64_t* tfull_bar = empty_bar + 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull_bar + 1);
   float* recv = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 256);   // [pk][128][rstride]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -77,16 +74,11 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
     tma_prefetch_desc(&tma_b);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], EPI_WARPS);
     }
-    mbar_init(tfull_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // Phase 1 of the cluster barrier = "every CTA of the cluster is running" (required before touching a peer's shared
   // memory); arrive now, wait only right before the first remote store so the wait hides behind the main loop.
   cluster_arrive_relaxed();
@@ -117,70 +109,43 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(TypeInfo<T>::umma_fmt, BM, BN);
+  } else if (warp >= 4) {
+    // ---------------------------------------------------------------- consumers: partial tile, then scatter it
+    pdl_wait();
+    const int wg = (warp - 4) >> 2;
+    float d[BN / 2];
+    if (my_kb > 0) {
       int s = 0;
       uint32_t ph = 0;
-      for (int i = 0; i < my_kb; ++i) {
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
-        const uint64_t da = umma_desc_k128(sa);
-        const uint64_t db = umma_desc_k128(sa + A_BYTES);
+      wg_mainloop<T, BN, BK>(d, smem, STAGE_BYTES, A_BYTES, STAGES, full_bar, empty_bar, s, ph, my_kb, wg, lane,
+                             [](const uint8_t*) {});
+    } else {
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) umma_f16(tmem_base, da + 2 * k, db + 2 * k, idesc, (i | k) != 0 ? 1u : 0u);
-        umma_commit(&empty_bar[s]);
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-      umma_commit(tfull_bar);
+      for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
     }
-  } else {
-    // ---------------------------------------------------------------- epilogue warps: scatter the partial tile
-    pdl_wait();
-    const int q = warp & 3;
-    const int row_t = q * 32 + lane;                 // tile row == TMEM lane
     const uint32_t recv_local = smem_u32(recv);
-    if (my_kb > 0) {
-      mbar_wait(tfull_bar, 0);
-      tc_fence_after();
-    }
-    __syncwarp();
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);       // fragment rows r0 and r0 + 8 of the tile
+    const int c = (lane & 3) * 2;
     cluster_wait();
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t v[32];
-      if (my_kb > 0) {
-        __syncwarp();
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c * 32, v);
-        tmem_ld_wait();
-      } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0u;
-      }
+    for (int unit = 0; unit < N_UNITS; ++unit) {                  // n8 block == 8-column unit
+      int owner = 0;                                              // largest j with first_unit(j) <= unit
+      while (owner + 1 < pk && sk_first_unit(owner + 1, N_UNITS, pk) <= unit) ++owner;
+      const int local_col = (unit - sk_first_unit(owner, N_UNITS, pk)) * 8 + c;
 #pragma unroll
-      for (int u4 = 0; u4 < 4; ++u4) {
-        const int unit = c * 4 + u4;
-        int owner = 0;                               // largest j with first_unit(j) <= unit
-        while (owner + 1 < pk && sk_first_unit(owner + 1, N_UNITS, pk) <= unit) ++owner;
-        const int local_col = (unit - sk_first_unit(owner, N_UNITS, pk)) * 8;
-        const uint32_t off = ((static_cast<uint32_t>(rank) * BM + row_t) * rstride + local_col) * 4u;
-        const uint32_t dst = mapa_shared(recv_local + off, static_cast<uint32_t>(owner));
-        st_cluster_f4(dst, __uint_as_float(v[u4 * 8 + 0]), __uint_as_float(v[u4 * 8 + 1]), __uint_as_float(v[u4 * 8 + 2]),
-                      __uint_as_float(v[u4 * 8 + 3]));
-        st_cluster_f4(dst + 16, __uint_as_float(v[u4 * 8 + 4]), __uint_as_float(v[u4 * 8 + 5]), __uint_as_float(v[u4 * 8 + 6]),
-                      __uint_as_float(v[u4 * 8 + 7]));
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t off = ((static_cast<uint32_t>(rank) * BM + r0 + 8 * h) * rstride + local_col) * 4u;
+        st_cluster_f2(mapa_shared(recv_local + off, static_cast<uint32_t>(owner)), d[4 * unit + 2 * h], d[4 * unit + 2 * h + 1]);
       }
     }
-    tc_fence_before();
   }
 
   __syncwarp();
-  if (warp < 2) cluster_wait();     // producer / MMA warps complete phase 1 here
+  if (warp < 4) cluster_wait();     // producer and idle warps complete phase 1 here
   // every partial of this cluster's tile is in its owner's receive buffer after this barrier
   cluster_sync_all();
 
-  if (warp >= 2) {
+  if (warp >= 4 && warp < 8) {
     const int q = warp & 3;
     const int row_t = q * 32 + lane;
     const int row = mb * BM + row_t;
@@ -248,12 +213,6 @@ gemm_splitk_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 static int sk_rstride(int bn, int pk) { return ((bn / 8 + pk - 1) / pk) * 8 + 4; }   // +4 floats: rows land in different banks
@@ -311,10 +270,9 @@ static int launch_splitk(const GemmArgs& a, int pk, cudaStream_t stream) {
   return launch_ok();
 }
 
-// Chooses a split for skinny GEMMs; returns 0 when the plain kernel should be used.  Measured on B200 inside CUDA-graph
-// replays (tools/bench_gemm.py, profiles/r01_gemm_decode_microbench.md): a cluster launch costs ~2 us more than a plain one
-// and clusters of >= 5 CTAs are 2-3x slower (GPC placement), so the split only pays when the per-CTA k-chain is long —
-// the down projections (K = 3424 / 4096: 16.3 -> 13.0 us with 3 x BN64).  Everything else stays on the plain kernel.
+// Chooses a split for skinny GEMMs; returns 0 when the plain kernel should be used.  A cluster launch costs more than a plain
+// one and large clusters are placed less freely, so the split is kept to <= 3 CTAs and used only when the per-CTA k-chain is
+// long (the decoder's down projections, K = 3424 / 4096).  Everything else stays on the plain kernel.
 int splitk_plan(const GemmArgs& a, int* bn_out) {
   if (a.out_f32 || a.group_k || a.M > 256 || a.swiglu) return 0;
   const int k_blocks = (a.K + 63) / 64;

@@ -45,7 +45,7 @@ __global__ void rmsnorm_kernel(const T* __restrict__ x, int ldx, const T* __rest
   // mode 0: Qwen2RMSNorm  y = w * T(x * rsqrt(mean + eps))
   // mode 1: SuryaADETRDecoderRMSNorm (adetr/decoder.py:29-47)  y = T(clamp(x * rsqrt(max(mean, eps)) * (1 + w)))
   float inv = mode ? rsqrtf(fmaxf(ss / static_cast<float>(H), eps)) : rsqrtf(ss / static_cast<float>(H) + eps);
-  const float tmax = sizeof(T) == 2 && TypeInfo<T>::umma_fmt == 0 ? 65504.f : 3.3895313892515355e38f;
+  const float tmax = sizeof(T) == 2 && !TypeInfo<T>::is_bf16 ? 65504.f : 3.3895313892515355e38f;
   for (int i = lane; i < nv; i += 32) {
     uint4 u = *reinterpret_cast<const uint4*>(xr + i * 8);
     uint4 wv = *reinterpret_cast<const uint4*>(w + i * 8);

@@ -64,7 +64,7 @@ struct AttnArgs {
 };
 int attn_varlen(const AttnArgs& a, cudaStream_t st);
 
-// k x k dense convolution (NHWC, implicit GEMM on tcgen05); weight [Cout, k*k*Cin] with K ordered (r, s, c).
+// k x k dense convolution (NHWC, implicit GEMM on wgmma); weight [Cout, k*k*Cin] with K ordered (r, s, c).
 struct ConvArgs {
   int dtype = DT_F16;
   const void* in = nullptr;      // [n_img, H, W, Cin]
@@ -76,12 +76,12 @@ struct ConvArgs {
 };
 int conv_igemm(const ConvArgs& a, cudaStream_t st);
 
-// FusedMBConv (conv_fmb.cu): 3x3 expand conv + Hardswish + 1x1 project (+ shortcut) as one back-to-back tcgen05 GEMM kernel.
+// FusedMBConv (conv_fmb.cu): 3x3 expand conv + Hardswish + 1x1 project (+ shortcut) as one back-to-back wgmma GEMM kernel.
 bool fmb_fused_ok(int Cin, int Cmid, int Cout, int ksize, int stride, int pad, int act1, int act2);
 int fmb_fused(int dtype, const void* in, const void* w1, const float* bias1, const void* w2, const float* bias2,
               const void* residual, void* out, int n_img, int H, int W, int Cin, int Cmid, int Cout, int stride, cudaStream_t st);
 
-// Fused decode head (det_head.cu): upsample + concat + fuse conv + ReLU + classifier + sigmoid in one tcgen05 kernel.
+// Fused decode head (det_head.cu): upsample + concat + fuse conv + ReLU + classifier + sigmoid in one wgmma kernel.
 bool det_head_fused_ok(int n_src, int CS, int n_out, int cin, int cout, const int* hs, const int* ws, int HO, int WO);
 int det_head_fused(int dtype, const void* const* srcs, const int* hs, const int* ws, const int* ch_off, int n_src, int CS,
                    const void* fuse_w, const float* fuse_bias, const void* cls_w, const void* cls_b, void* logits, int B, int HO,

@@ -41,9 +41,8 @@ struct sb_rec_engine {
   float* am_val = nullptr; int* am_idx = nullptr; float* am_sum = nullptr;
   int am_ld = 0, am_bn = 0;
   // gemm_chain (o_proj -> gate/up -> down -> next qkv in one persistent launch): barrier counters + switch.  OFF by default:
-  // measured 50.7 us per layer chain vs 46.4 us for the four PDL-chained launches (profiles/r02_chain_timeline.md) — each phase
-  // still pays ~1.5 us first-tile latency + ~2 us grid barrier, and the down projection loses its split-K kernel.  $SB_CHAIN=1
-  // or sb_rec_set_option("chain", 1) turns it on.
+  // each phase still pays its first-tile latency plus a grid barrier, and the down projection loses its split-K kernel (not
+  // re-measured on H100).  $SB_CHAIN=1 or sb_rec_set_option("chain", 1) turns it on.
   unsigned int* chain_bar = nullptr;
   int use_chain = 0;
   int qkv_w_enc = 0, qkv_w_dec = 0;
@@ -165,9 +164,8 @@ static int run_heads(sb_rec_engine* e, void* hidden, int rows, const HeadOut& o,
   a.M = rows; a.N = c.vocab; a.K = D;
   a.bias = static_cast<const float*>(e->W(SB_RW_LM_BIAS));
   a.w_constant = 1;
-  // 1/rms of the final norm: separate pass + rowscale rather than the in-kernel sum of squares — this GEMM runs several tiles
-  // per CTA, and the in-kernel pass would serialise each tile's main loop behind the previous tile's epilogue (lm_head
-  // 63 vs 48 us, profiles/r02_decode_parts.md)
+  // 1/rms of the final norm: separate pass + rowscale rather than the in-kernel sum of squares — this GEMM has hundreds of
+  // column tiles per row block, and the in-kernel pass would recompute the rows' sum of squares for every one of them
   CK(row_rstd(c.dtype, hidden, D, e->rs, rows, D, c.rms_eps, nullptr, st));
   a.rowscale = e->rs;
   a.am_val = e->am_val; a.am_idx = e->am_idx; a.am_sum = e->am_sum; a.am_ld = e->am_ld;

@@ -1,9 +1,9 @@
-"""Drop-in binding: run the reference's *unmodified* predictors on top of the B200 engines.
+"""Drop-in binding: run the reference's *unmodified* predictors on top of the CUDA engines.
 
 The reference has no plugin/FFI seam; a predictor reaches its network through `self.model` / `self.processor`, which
 `BasePredictor.__init__` obtains from `self.model_loader_cls(checkpoint)` (surya/common/predictor.py:20-29).  The binding
 therefore consists of
-  * a loader class (`loader_for`) that hands out a B200 model mirror and the caller's processor — the predictor
+  * a loader class (`loader_for`) that hands out an engine model mirror and the caller's processor — the predictor
     subclass only overrides the `model_loader_cls` class attribute, every method of the reference class runs as is;
   * for recognition, `install()`: RecognitionPredictor.prefill constructs its KV cache itself from the module-level
     name `ContinuousBatchingCache` (surya/recognition/__init__.py:41-44, 391-395); that name is re-pointed at
@@ -60,7 +60,7 @@ def _subclass(base, model, processor, name):
 
 
 def recognition_predictor(model: B200SuryaModel, processor: Any, **kw):
-    """`RecognitionPredictor` (reference class, unmodified) whose model is the B200 engine mirror."""
+    """`RecognitionPredictor` (reference class, unmodified) whose model is the engine mirror."""
     mod = install()
     return _subclass(mod.RecognitionPredictor, model, processor, "B200RecognitionPredictor")(**kw)
 

@@ -1,6 +1,6 @@
 """Layout path: Donut-Swin encoder + ADETR box decoder on the CUDA kernels, behind the call surface LayoutPredictor uses.
 
-  * LayoutEngine        packed weights + forward passes built from libsurya_b200.so ops (tcgen05 GEMMs for every Linear,
+  * LayoutEngine        packed weights + forward passes built from libsurya_b200.so ops (wgmma GEMMs for every Linear,
                         swin_window_attn, layernorm, decode_attn / attn_single_query, ...); round 1 drives the layer loops
                         from Python (correctness first), the kernels are the same ones the C++ engines use
   * B200LayoutModel     quacks like the model LayoutPredictor touches (surya/layout/__init__.py:83-123, 222):

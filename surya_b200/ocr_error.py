@@ -1,15 +1,15 @@
-"""ocr_error path on B200 (SURVEY §8 f4): DistilBertForSequenceClassification forward + the predictor's label loop.
+"""ocr_error path on the GPU (SURVEY §8 f4): DistilBertForSequenceClassification forward + the predictor's label loop.
 
 Reference: surya/ocr_error/model/encoder.py:48-91 (Embeddings), :133-195 (MultiHeadSelfAttention), :381-399 (FFN), :408-463
 (TransformerBlock), :731-763 (classification head), surya/ocr_error/__init__.py:19-62 (OCRErrorPredictor).  The tokenizer
 (surya/ocr_error/tokenizer.py) is host string processing and stays the reference's own.
 
-B200-first layout: the right-padded [B, L] batch the tokenizer produces (padding="longest") is PACKED on the host — only real
+GPU-first layout: the right-padded [B, L] batch the tokenizer produces (padding="longest") is PACKED on the host — only real
 tokens become rows, every text is one segment of the block-diagonal attention kernel, so no pad position is ever embedded,
 projected or attended (the reference computes them and masks the keys, encoder.py:171-175).  Per layer: one fused q/k/v GEMM
-(tcgen05), `attn_varlen` (non-causal), out_lin GEMM with the residual in its epilogue, LayerNorm, lin1 GEMM + erf-GELU epilogue,
+(wgmma), `attn_varlen` (non-causal), out_lin GEMM with the residual in its epilogue, LayerNorm, lin1 GEMM + erf-GELU epilogue,
 lin2 GEMM + residual, LayerNorm; then the [CLS] rows are gathered, pre_classifier GEMM + ReLU epilogue and the 2-way classifier.
-Everything launches hand-written sm_100a kernels through the C ABI (`ops.py`); there is no PyTorch fallback.
+Everything launches hand-written sm_90a kernels through the C ABI (`ops.py`); there is no PyTorch fallback.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """Torch-tensor wrappers over the op-level C ABI (include/surya_b200.h).
 
-torch is used for device memory and streams only; every function launches hand-written sm_100a kernels from
+torch is used for device memory and streams only; every function launches hand-written sm_90a kernels from
 libsurya_b200.so on torch's current CUDA stream and raises if the library or a GPU is missing.
 """
 from __future__ import annotations

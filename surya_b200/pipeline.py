@@ -1,5 +1,5 @@
 """BASELINE config 5: the `ocr_text` data flow (surya/scripts/ocr_text.py:32-38 -> RecognitionPredictor.__call__,
-surya/recognition/__init__.py:773-942) on the B200 engines: detect -> boxes -> crop -> width-sorted recognition.
+surya/recognition/__init__.py:773-942) on the CUDA engines: detect -> boxes -> crop -> width-sorted recognition.
 
   pages (uint8)  --H2D 3 B/px-->  normalise + EfficientViT + post-processing front half (device)
                  --D2H 3 B/px-->  connected components / min-area rectangles (host OpenCV, thread pool; heatmap.py:27-107)
@@ -103,7 +103,7 @@ def slice_polygon(image: np.ndarray, poly: Sequence[Sequence[int]]) -> np.ndarra
 
 
 class OcrPipeline:
-    """detect -> crop -> recognise over the B200 engines.  `run(pages)` takes uint8 pages [N, H, W, 3] (H, W = the detection
+    """detect -> crop -> recognise over the CUDA engines.  `run(pages)` takes uint8 pages [N, H, W, 3] (H, W = the detection
     processor size) and returns (lines grouped per page, timing breakdown in seconds)."""
 
     def __init__(self, det: DetEngine, rec: RecEngine, rec_batch: int = 256, max_tokens: int = 128, det_chunk: int = 16,

@@ -1,4 +1,4 @@
-"""pytest configuration: `gpu` marks tests that need a real B200; everything else runs on CPU."""
+"""pytest configuration: `gpu` marks tests that need a real H100; everything else runs on CPU."""
 import os
 import sys
 from pathlib import Path
@@ -11,7 +11,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -368,7 +368,7 @@ def _head_logits(size, B, seed):
 @pytest.mark.parametrize("size", [(512, 512), (320, 448)])
 @pytest.mark.parametrize("switch", ["SB_DET_FUSED_HEAD", "SB_FMB_FUSED"])
 def test_fused_kernels_equal_unfused_ops(built_lib, switch, size, tmp_path):
-    """The fused tcgen05 kernels against the op sequences they replace (switch = 1 / 0, read once per process, hence the subprocesses):
+    """The fused wgmma kernels against the op sequences they replace (switch = 1 / 0, read once per process, hence the subprocesses):
       SB_DET_FUSED_HEAD  det_head.cu (upsample + concat + fuse conv + ReLU + classifier + sigmoid) vs upsample_cat -> gemm ->
                          classifier: same rounding points, only the fp32 summation order of the 512-long classifier dot differs;
       SB_FMB_FUSED       conv_fmb.cu (3x3 expand + Hardswish + 1x1 project + shortcut, back-to-back GEMM) vs conv_igemm -> gemm:

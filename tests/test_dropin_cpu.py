@@ -1,12 +1,11 @@
 """Drop-in boundary (SURVEY.md §8b) on CPU.
 
-Two kinds of tests:
-  * with /root/reference mounted (build container): the reference's UNMODIFIED predictor classes run on top of the B200 model
-    mirrors (B200SuryaModel + SlotCache, B200EfficientViT) bound through surya_b200.dropin; the engine behind the mirror is the
-    CPU oracle (oracle/ref_predictors.py) because this container has no GPU.  These are the `test_reference_*predictor_dropin*`
-    tests; they skip on the GPU box, where /root/reference does not exist.
-  * everywhere: the committed trace of such a predictor run (tests/golden/rec_predictor_trace.pt) is replayed against the same
-    boundary code without the reference.  tests/test_rec_gpu.py replays the same trace against the CUDA engine.
+The reference's UNMODIFIED predictor classes were run on top of the model mirrors (B200SuryaModel + SlotCache, B200EfficientViT)
+bound through surya_b200.dropin, with the CPU oracle as the engine (oracle/make_golden.py, targets `trace` and `pins`); what they
+returned is committed under tests/golden/ and these tests check the product against it:
+  * the predictor trace (tests/golden/rec_predictor_trace.pt) is replayed against the same boundary code;
+    tests/test_rec_gpu.py replays the same trace against the CUDA engine;
+  * the reference's detection post-processing, pipeline host stages and predictor outputs (tests/golden/reference_pins.pt).
 """
 from pathlib import Path
 
@@ -15,11 +14,13 @@ import pytest
 import torch
 
 from oracle import rec_oracle as O
-from oracle import ref_shim
 
 ROOT = Path(__file__).resolve().parent.parent
 GOLDEN = ROOT / "tests" / "golden"
-needs_reference = pytest.mark.skipif(not ref_shim.available(), reason="/root/reference is only mounted in the build container")
+
+
+def _pins():
+    return torch.load(GOLDEN / "reference_pins.pt", weights_only=False)
 
 
 def _tile_fn(cfg):
@@ -29,13 +30,12 @@ def _tile_fn(cfg):
     return fn
 
 
-@needs_reference
 def test_reference_recognition_predictor_dropin_cpu():
     """RecognitionPredictor.prediction_loop (reference code, unmodified: prefill with its own `ContinuousBatchingCache()`,
     merge, mask/position bookkeeping, maybe_trim_cache_padding, stop rules, `del self.kv_cache`) over B200SuryaModel +
-    SlotCache: every crop must decode exactly as the oracle decodes it alone, merges must see both offset signs, and all KV
-    slots must be back in the engine afterwards."""
-    from oracle import ref_predictors as RP
+    SlotCache, as committed in tests/golden/rec_predictor_trace.pt: every crop must have decoded exactly as the oracle decodes
+    it alone, and the run must have seen merges of both offset signs and a trim.  (Slots coming back after the loop is checked
+    by the replay test.)"""
     from oracle.make_golden import trace_crops
     from surya_b200.config import tiny_rec
     from surya_b200.synth import rec_state_dict
@@ -43,23 +43,17 @@ def test_reference_recognition_predictor_dropin_cpu():
     cfg = tiny_rec()
     sd = rec_state_dict(cfg, seed=0)
     crops = trace_crops()
-    events, tokens, bboxes, scores, eng = RP.record_rec_trace(cfg, sd, crops, batch_size=3, max_tokens=10, min_trim_length=2)
+    g = torch.load(GOLDEN / "rec_predictor_trace.pt", weights_only=False)
+    events, tokens, bboxes, scores = g["events"], g["tokens"], g["bboxes"], g["scores"]
     offsets = [e["offset"] for e in events if e["kind"] == "merge"]
     assert any(o > 0 for o in offsets) and any(o < 0 for o in offsets), offsets
     assert any(e["kind"] == "trim" for e in events)
-    assert len(eng.free_slots) == eng.max_slots, "KV slots leaked by the predictor run"
+    assert len(tokens) == len(crops)
     for i, crop in enumerate(crops):
         otok, osc, obox, hist = O.greedy_decode(sd, cfg, O.build_batch([crop], cfg), 10, torch.float32, stop_rules=True)
         assert tokens[i] == hist[0], f"crop {i}: {tokens[i]} vs oracle {hist[0]}"
         assert np.allclose(scores[i], osc[0, : len(hist[0])].numpy(), atol=1e-5)
-        assert torch.equal(bboxes[i, : len(hist[0])].long(), obox[0, : len(hist[0])])
-    # the committed fixture is what this run produces
-    g = torch.load(GOLDEN / "rec_predictor_trace.pt")
-    assert g["tokens"] == tokens
-    assert [e["kind"] for e in g["events"]] == [e["kind"] for e in events]
-    # a second loop on the same engine must find every slot free again (ADVICE r1: slot leak through `del self.kv_cache`)
-    events2, tokens2, *_ = RP.record_rec_trace(cfg, sd, crops[:4], batch_size=3, max_tokens=4)
-    assert tokens2 == [t[:4] for t in tokens[:4]]
+        assert torch.equal(torch.as_tensor(bboxes[i])[: len(hist[0])].long(), obox[0, : len(hist[0])])
 
 
 def test_predictor_trace_replay_cpu():
@@ -140,123 +134,83 @@ def test_dropin_install_is_reversible():
     assert L("ckpt").model("cpu", None) == "m" and L().processor() == "p"
 
 
-@needs_reference
 def test_reference_detection_predictor_config1_and_dropin_cpu():
     """BASELINE config 1: one 1024x1024 synthetic page (the reference's own conftest page) through the reference
-    DetectionPredictor on CPU — (a) with the reference's own model (plumbing check of the stock path), (b) with
-    B200EfficientViT over the oracle engine bound through surya_b200.dropin.  Same heatmaps -> same TextDetectionResult."""
+    DetectionPredictor with the reference's own model, as committed in tests/golden/reference_pins.pt, against B200EfficientViT over
+    the oracle engine: the heat maps handed to the post-processing are the same up to fp32 noise, and the product's host chain
+    (bilinear up-sampling, dynamic thresholds, boxes, polygons) gives the predictor's TextDetectionResult boxes."""
+    import torch.nn.functional as F
+
+    from oracle import det_oracle as D
     from oracle import ref_predictors as RP
-    from surya_b200 import dropin
     from surya_b200.config import det_default
-    from surya_b200.detection import B200EfficientViT
-    from surya_b200.synth import det_state_dict
+    from surya_b200.detection import B200EfficientViT, text_boxes_from_front
+    from surya_b200.pipeline import page_polygons
+    from surya_b200.synth import det_normalize, det_state_dict
 
-    RP.install_predictors()
-    from surya.detection import DetectionPredictor
-    from surya.detection.schema import TextDetectionResult
-
+    pin = _pins()["det_config1"]
+    assert pin["image_bbox"] == [0, 0, 1024, 1024]
     cfg = det_default()
     sd = det_state_dict(cfg, seed=0)
-    ref_model = ref_shim.build_reference_det_model(cfg, sd)
-    proc = RP.synthetic_det_processor(1024)
-    page = RP.conftest_page(1024)
-
-    Stock = type("StockDetectionPredictor", (DetectionPredictor,), {"model_loader_cls": dropin.loader_for(ref_model, proc)})
-    stock = Stock(device="cpu", dtype=torch.float32)
-    stock.disable_tqdm = True
-    res_ref = stock([page])
-    assert len(res_ref) == 1 and isinstance(res_ref[0], TextDetectionResult)
-    assert res_ref[0].image_bbox == [0, 0, 1024, 1024]
-
-    pred = dropin.detection_predictor(B200EfficientViT(RP.OracleDetEngine(cfg, sd)), proc, device="cpu", dtype=torch.float32)
-    pred.disable_tqdm = True
-    res = pred([page], include_maps=False)
-    assert len(res) == 1 and res[0].image_bbox == [0, 0, 1024, 1024]
-    assert [b.polygon for b in res[0].bboxes] == [b.polygon for b in res_ref[0].bboxes]
-    # and the heat maps the two models hand to the post-processing are the same tensor up to fp32 noise
-    x = torch.from_numpy(proc(np.asarray(page, dtype=np.uint8))["pixel_values"][0])[None]
-    with torch.inference_mode():
-        a = ref_model(pixel_values=x).logits
-    b = B200EfficientViT(RP.OracleDetEngine(cfg, sd))(pixel_values=x).logits
-    assert (a - b).abs().max().item() < 1e-4
+    x = det_normalize(np.asarray(RP.conftest_page(1024), dtype=np.uint8)[None])
+    assert abs(x.double().sum().item() - pin["page_checksum"].item()) < 1e-3 * x.numel() ** 0.5
+    logits = B200EfficientViT(RP.OracleDetEngine(cfg, sd))(pixel_values=x).logits.float()
+    assert tuple(logits.shape) == pin["logits_shape"]
+    assert (logits.reshape(-1)[pin["logit_idx"]] - pin["logit_sample"]).abs().max().item() < 1e-4
+    up = F.interpolate(logits, size=[1024, 1024], mode="bilinear", align_corners=False)[0, 0].numpy()
+    tt, low, _ = D.dynamic_thresholds(up)
+    boxes, conf = text_boxes_from_front(up, (up > low).astype(np.uint8), float(tt), float(low))
+    polys, _ = page_polygons(boxes, conf, (1024, 1024), (1024, 1024))
+    assert len(polys) >= 1
+    assert [[[float(v) for v in pt] for pt in p] for p in polys] == pin["polygons"]
 
 
-@needs_reference
 def test_det_postprocess_oracle_pinned_to_reference():
-    """oracle.det_oracle.dynamic_thresholds / detect_boxes and the product's text_boxes_from_front against the reference's own
-    surya.detection.heatmap functions on synthetic heat maps (smooth blobs of text-line shape): identical thresholds, boxes and
-    confidences."""
-    import cv2
-
+    """oracle.det_oracle.dynamic_thresholds / detect_boxes and the product's text_boxes_from_front against what the reference's own
+    surya.detection.heatmap functions returned on the same synthetic heat maps (smooth blobs of text-line shape; committed in
+    tests/golden/reference_pins.pt): identical thresholds, boxes and confidences."""
     from oracle import det_oracle as D
-    from oracle import ref_predictors as RP
+    from oracle.make_golden import det_heatmap_trials
     from surya_b200.detection import text_boxes_from_front
 
-    RP.install_predictors()
-    from surya.detection.heatmap import detect_boxes, get_dynamic_thresholds
-
-    rng = np.random.default_rng(5)
-    for trial in range(3):
-        m = np.zeros((512, 640), np.float32)
-        for _ in range(25):
-            x, y = int(rng.integers(0, 560)), int(rng.integers(0, 480))
-            w, h = int(rng.integers(30, 200)), int(rng.integers(6, 24))
-            m[y:y + h, x:x + w] = rng.uniform(0.3, 1.0)
-        m = cv2.GaussianBlur(m, (0, 0), 2.0).astype(np.float16).astype(np.float32)     # 16-bit-valued like the engine's maps
-        tt_ref, low_ref = get_dynamic_thresholds(m, 0.6, 0.35)
+    maps, _ = det_heatmap_trials(5, 3)
+    for m, ref in zip(maps, _pins()["det_postprocess"]):
         tt, low, _ = D.dynamic_thresholds(m)
-        assert float(tt) == float(tt_ref) and float(low) == float(low_ref)
-        ref_boxes, ref_conf = detect_boxes(m, 0.6, 0.35)
+        assert float(tt) == ref["tt"] and float(low) == ref["low"]
         boxes, conf = D.detect_boxes(m)
         pboxes, pconf = text_boxes_from_front(m.astype(np.float16), (m > low).astype(np.uint8), float(tt), float(low))
-        assert len(ref_boxes) == len(boxes) == len(pboxes) and len(boxes) > 3
-        for a, b, c in zip(ref_boxes, boxes, pboxes):
-            assert np.array_equal(a, b) and np.array_equal(a, c)
-        assert np.allclose(ref_conf, conf, atol=0) and np.allclose(ref_conf, pconf, atol=1e-7)
+        assert len(ref["boxes"]) == len(boxes) == len(pboxes) and len(boxes) > 3
+        for a, b, c in zip(ref["boxes"], boxes, pboxes):
+            assert np.array_equal(a.numpy(), b) and np.array_equal(a.numpy(), c)
+        assert np.allclose(ref["conf"], conf, atol=0) and np.allclose(ref["conf"], pconf, atol=1e-7)
 
 
-@needs_reference
 def test_pipeline_host_stages_pinned_to_reference():
-    """surya_b200.pipeline.page_polygons / slice_polygon against the reference's get_and_clean_boxes + parallel_get_boxes expansion
-    (surya/detection/heatmap.py:125-175) and slice_polys_from_image (surya/input/processing.py:57-101) on synthetic heat maps."""
-    import cv2
+    """surya_b200.pipeline.page_polygons / slice_polygon against what the reference's get_and_clean_boxes + parallel_get_boxes
+    expansion (surya/detection/heatmap.py:125-175) and slice_polys_from_image (surya/input/processing.py:57-101) returned on the
+    same synthetic heat maps and pages (committed in tests/golden/reference_pins.pt; crops compared through their SHA-256)."""
+    import hashlib
 
     from oracle import det_oracle as D
-    from oracle import ref_predictors as RP
+    from oracle.make_golden import det_heatmap_trials
     from surya_b200.detection import text_boxes_from_front
     from surya_b200.pipeline import page_polygons, slice_polygon
 
-    RP.install_predictors()
-    from surya.detection.heatmap import get_and_clean_boxes
-    from surya.input.processing import slice_polys_from_image
-    from surya.settings import settings
-
-    rng = np.random.default_rng(9)
-    for trial in range(3):
-        H, W = 512, 640
-        m = np.zeros((H, W), np.float32)
-        for _ in range(20):
-            x, y = int(rng.integers(0, W - 60)), int(rng.integers(0, H - 30))
-            w, h = int(rng.integers(30, 220)), int(rng.integers(6, 30))
-            m[y:y + h, x:x + w] = rng.uniform(0.3, 1.0)
-        m[40:60, 100:300] = 0.9
-        m[44:56, 150:250] = 0.95                                   # a box contained in another one
-        m = cv2.GaussianBlur(m, (0, 0), 1.5).astype(np.float16).astype(np.float32)
+    for trial, ref in enumerate(_pins()["pipeline_host"]):
+        m = det_heatmap_trials(9 * 1000 + trial, 1, boxes=20, blur=1.5, nested=True)[0][0]
+        H, W = m.shape
         img_size = (W * 2, H * 2) if trial == 1 else (W, H)       # also exercise the rescale path
-        ref = get_and_clean_boxes(m, [W, H], img_size)
-        for box in ref:
-            if box.height < 3 * box.width:
-                box.expand(x_margin=0, y_margin=settings.DETECTOR_BOX_Y_EXPAND_MARGIN)
-                box.fit_to_bounds([0, 0, img_size[0], img_size[1]])
+        assert tuple(ref["img_size"]) == img_size
         tt, low, _ = D.dynamic_thresholds(m)
         boxes, conf = text_boxes_from_front(m, (m > low).astype(np.uint8), float(tt), float(low))
         polys, pconf = page_polygons(boxes, conf, img_size, (W, H))
-        assert len(polys) == len(ref) and len(polys) > 3
-        for p, r, c in zip(polys, ref, pconf):
-            assert [[float(v) for v in pt] for pt in p] == [[float(v) for v in pt] for pt in r.polygon], (p, r.polygon)
-            assert abs(c - r.confidence) < 1e-6
+        assert len(polys) == len(ref["polygons"]) and len(polys) > 3
+        for p, r, c, rc in zip(polys, ref["polygons"], pconf, ref["conf"]):
+            assert [[float(v) for v in pt] for pt in p] == r, (p, r)
+            assert abs(c - rc) < 1e-6
         if trial != 1:
-            page = rng.integers(0, 256, size=(H, W, 3)).astype(np.float32)
-            ref_slices = slice_polys_from_image(page, [[[int(v) for v in pt] for pt in r.polygon] for r in ref])
-            for p, rs in zip(polys, ref_slices):
-                assert np.array_equal(slice_polygon(page, p), rs)
+            page = np.random.default_rng(9 * 1000 + trial).integers(0, 256, size=(H, W, 3)).astype(np.float32)
+            for p, (shape, dtype, digest) in zip(polys, ref["slices"]):
+                sl = np.ascontiguousarray(slice_polygon(page, p))
+                assert (tuple(sl.shape), str(sl.dtype)) == (tuple(shape), dtype)
+                assert hashlib.sha256(sl.tobytes()).hexdigest() == digest

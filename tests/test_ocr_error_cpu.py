@@ -11,14 +11,12 @@ import torch
 import torch.nn.functional as F
 
 from oracle import ocr_error_oracle as E
-from oracle import ref_shim
 from surya_b200 import _lib
 from surya_b200 import ocr_error as OE
 from surya_b200.config import ocr_error_default, ocr_error_tiny
 from surya_b200.synth import ocr_error_state_dict, ocr_error_synthetic_batch
 
 GOLDEN = Path(__file__).parent / "golden"
-needs_reference = pytest.mark.skipif(not ref_shim.available(), reason="/root/reference is only mounted in the build container")
 
 
 @pytest.mark.parametrize("kind", ["tiny", "default"])
@@ -148,37 +146,23 @@ class _HashTokenizer:
         return SimpleNamespace(input_ids=ids, attention_mask=mask)
 
 
-@needs_reference
 def test_reference_ocr_error_predictor_dropin_cpu():
-    """The reference's UNMODIFIED OCRErrorPredictor (a) over its own DistilBertForSequenceClassification and (b) over the
-    B200DistilBert mirror bound through surya_b200.dropin (the network behind the mirror is the CPU oracle here: no GPU in this
-    container) — same labels for the same texts, batches of 3 with a ragged tail."""
-    from surya_b200 import dropin
+    """The reference's UNMODIFIED OCRErrorPredictor over its own DistilBertForSequenceClassification labelled these texts in batches of
+    3 with a ragged tail (committed in tests/golden/reference_pins.pt); the B200DistilBert mirror (the network behind it is the CPU
+    oracle here) through detect_errors — the predictor's batching after tokenisation — must give the same labels."""
+    from oracle.make_golden import ocr_error_texts
 
-    ref_shim.install()
-    from surya.ocr_error import OCRErrorPredictor
-    from surya.ocr_error.schema import OCRErrorDetectionResult
-
+    pin = torch.load(GOLDEN / "reference_pins.pt", weights_only=False)["ocr_error_predictor"]
     cfg = ocr_error_tiny()
     sd = ocr_error_state_dict(cfg, seed=0)
-    rng = np.random.default_rng(0)
-    words = [f"w{i}" for i in range(300)]
-    texts = [" ".join(rng.choice(words, size=int(rng.integers(2, 30)))) for _ in range(8)]
-    tok = _HashTokenizer(cfg)
-
-    ref_model = ref_shim.build_reference_ocr_error_model(cfg, sd)
-    Stock = type("StockOCRErrorPredictor", (OCRErrorPredictor,), {"model_loader_cls": dropin.loader_for(ref_model, tok)})
-    stock = Stock(device="cpu", dtype=torch.float32)
-    stock.disable_tqdm = True
-    res_ref = stock(texts, batch_size=3)
-    assert isinstance(res_ref, OCRErrorDetectionResult) and len(res_ref.labels) == len(texts)
+    texts = ocr_error_texts()
+    assert texts == pin["texts"]
+    enc = _HashTokenizer(cfg)(texts)
 
     mirror = object.__new__(OE.B200DistilBert)
     mirror.config = mirror.cfg = cfg
     mirror.dtype, mirror.device = torch.float32, torch.device("cpu")
     mirror.forward_packed = lambda plan: E.forward(sd, cfg, *_unpack(plan, cfg))
-    pred = dropin.ocr_error_predictor(mirror, tok, device="cpu", dtype=torch.float32)
-    pred.disable_tqdm = True
-    res = pred(texts, batch_size=3)
-    assert res.labels == res_ref.labels and res.texts == texts
-    assert len(set(res.labels)) == 2, res.labels
+    labels = OE.detect_errors(mirror, enc.input_ids, enc.attention_mask, batch_size=3)
+    assert labels == pin["labels"]
+    assert len(set(labels)) == 2, labels

@@ -88,10 +88,8 @@ def test_gemm_epilogue(built_lib, dtype, act):
 @pytest.mark.parametrize("M,N,K,act,res", [(80000, 1024, 256, "hardswish", False), (75011, 512, 128, "gelu", True),
                                            (76800, 256, 192, "relu", False)])
 def test_gemm_two_ctas_per_sm_config(built_lib, dtype, M, N, K, act, res):
-    """The 128 x 128, 2-stage, two-CTAs-per-SM configuration for short-K GEMMs with an activation (gemm_tcgen05.cu two_cta_ok,
-    opt-in with SB_GEMM_2CTA=1 because it measured slower): bit-identical to a forced 128 x 256 tile (same per-element arithmetic,
-    same k order) and right against the fp32 restatement.  Without the switch this compares the default heuristic with the forced
-    tile, which must be bit-identical too."""
+    """Short-K GEMMs with an activation (detection's 1x1 expand convs): the default tile heuristic must be bit-identical to a
+    forced 128 x 256 tile (same per-element arithmetic, same k order) and right against the fp32 restatement."""
     from surya_b200 import ops
 
     g = torch.Generator(device="cuda").manual_seed(M % 97 + N + K)
@@ -584,7 +582,7 @@ def test_decode_attn_v2_variant_in_subprocess(built_lib):
                                        (16, 1536, 1024, "none"), (1, 20, 1024, "none")])
 def test_gemm_skinny_path(built_lib, dtype, M, N, K, epi):
     """M <= 16 routes to the mma.sync kernel (gemm_skinny.cu): against the fp32 restatement with the output roundings, and
-    against the tcgen05 kernel (forced tile width) to a few ulp — the two paths sum in different orders."""
+    against the wgmma kernel (forced tile width) to a few ulp — the two paths sum in different orders."""
     from surya_b200 import ops
 
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
@@ -607,4 +605,4 @@ def test_gemm_skinny_path(built_lib, dtype, M, N, K, epi):
     _close(got, ref, dtype, ulps=4.0 if epi == "geglu" else 2.0, what="skinny gemm", scale=lin if res is not None else None)
     if N % 8 == 0 and epi != "geglu":
         tc = ops.gemm(a, w, bias=bias, residual=res, act=act, force_bn=32)
-        _close(got, tc, dtype, ulps=2.0, what="skinny vs tcgen05", scale=lin if res is not None else None)
+        _close(got, tc, dtype, ulps=2.0, what="skinny vs wgmma", scale=lin if res is not None else None)

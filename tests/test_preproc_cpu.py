@@ -58,21 +58,23 @@ def test_preprocess_plan():
 
 
 def test_crop_chain_pinned_to_the_reference_processor():
-    """The restatement against the reference's OWN SuryaOCRProcessor (scale_to_fit + _process_and_tile, imported unmodified from
-    /root/reference; skipped where it is not mounted): same grids, tiles equal to float32 rounding of the OpenCV resizes."""
-    from oracle import ref_shim
-    if not ref_shim.available():
-        pytest.skip("/root/reference is only mounted in the build container")
-    from oracle import ref_predictors as RP
+    """The restatement against what the reference's OWN SuryaOCRProcessor (scale_to_fit + _process_and_tile) returned for the same
+    seeded crops (committed in tests/golden/reference_pins.pt: grids, per-tile-row sums and a seeded sample of the tiles): same
+    grids, tiles equal to float32 rounding of the OpenCV resizes."""
+    from pathlib import Path
 
-    RP.install_predictors()
+    import torch
+
+    from oracle.make_golden import PREPROC_SIZES
+
+    pins = torch.load(Path(__file__).parent / "golden" / "reference_pins.pt", weights_only=False)["preproc"]
     cfg = tiny_rec()
-    proc = RP.synthetic_ocr_processor(cfg)
     rng = np.random.default_rng(11)
-    for h, w in ((48, 512), (40, 300), (300, 2000), (20, 60), (56, 560), (97, 1403)):
+    tol = 2 * TOL_255 / 255 / 0.224
+    assert [tuple(p["size"]) for p in pins] == list(PREPROC_SIZES)
+    for (h, w), pin in zip(PREPROC_SIZES, pins):
         crop = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
-        img = proc.scale_to_fit(np.asarray(crop, dtype=np.float32), (1024, 256))
-        ref_tiles, ref_grid = proc._process_and_tile(img)
         tiles, grid = P.process_crop(crop, cfg.vision_encoder.patch_size, cfg.merge_size)
-        assert tuple(int(g) for g in ref_grid) == tuple(grid)
-        assert np.abs(tiles - ref_tiles.numpy()).max() <= 2 * TOL_255 / 255 / 0.224, (h, w)
+        assert tuple(pin["grid"]) == tuple(grid) and tuple(pin["shape"]) == tiles.shape
+        assert np.abs(tiles.reshape(-1)[pin["idx"].numpy()] - pin["sample"].numpy()).max() <= tol, (h, w)
+        assert np.abs(tiles.astype(np.float64).sum(1) - pin["row_sums"].numpy()).max() <= tol * tiles.shape[1], (h, w)

@@ -1,4 +1,4 @@
-"""In-kernel timeline of one CTA of the tcgen05 GEMM (globaltimer stamps): where do the microseconds of a small
+"""In-kernel timeline of one CTA of the wgmma GEMM (globaltimer stamps): where do the microseconds of a small
 decode-step GEMM go?  Usage (GPU box): python tools/gemm_timeline.py"""
 import ctypes
 import sys

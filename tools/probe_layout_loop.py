@@ -1,5 +1,5 @@
 import sys, time, torch
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, str(__import__("pathlib").Path(__file__).resolve().parent.parent))
 from surya_b200.config import layout_default, table_default
 from surya_b200.layout import LayoutEngine, layout_greedy, table_greedy
 from surya_b200.synth import adetr_layout_state_dict, adetr_table_state_dict, layout_synthetic_pages, swin_state_dict, table_query_tokens
