@@ -42,22 +42,16 @@ __global__ void __launch_bounds__(384, 1)
 fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_w1,
                  const __grid_constant__ CUtensorMap tma_w2, const FmbParams fp) {
   constexpr int TW = 16, TH = 8, CH = 128;                           // mid-channel chunk
-  // Cin = 32 (BKC == 32): the nine tap tiles of a pixel tile stay RESIDENT for all mid-channel chunks (one 64-byte-row TMA box each per
-  // tile instead of one per chunk) and W1 is streamed in [128 x 64] boxes that span a PAIR of taps (128-byte rows), which cuts the
-  // TMA line count per tile from 9216 to 3456.
-  constexpr bool RES_A = (BKC == 32);
   constexpr uint32_t A1_BYTES = 128 * BKC * 2;
-  constexpr uint32_t W1_BYTES = RES_A ? CH * 64 * 2 : CH * BKC * 2;
-  constexpr uint32_t S1_BYTES = RES_A ? W1_BYTES : A1_BYTES + W1_BYTES;
-  constexpr uint32_t RESA_BYTES = RES_A ? 9 * A1_BYTES : 0;
+  constexpr uint32_t W1_BYTES = CH * BKC * 2;
+  constexpr uint32_t S1_BYTES = A1_BYTES + W1_BYTES;
   constexpr uint32_t A2_KB_BYTES = 64 * 64 * 2;                      // one 64-channel k-block of a warpgroup's A2 tile (8 KB)
   constexpr uint32_t A2_WG_BYTES = 2 * A2_KB_BYTES;                  // 64 pixels x 128 mid channels
   constexpr uint32_t W2_KB_BYTES = COUT * 64 * 2, W2_BYTES = 2 * W2_KB_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // array + offset keeps the shared address space (STS / LDS, not generic ST / LD)
-  uint8_t* s_ra = smem;                                             // resident tap tiles (Cin = 32 only)
-  uint8_t* s_1 = s_ra + RESA_BYTES;
+  uint8_t* s_1 = smem;
   uint8_t* s_a2 = s_1 + STAGES * S1_BYTES;
   uint8_t* s_w2 = s_a2 + 2 * A2_WG_BYTES;
   float* s_b1 = reinterpret_cast<float*>(s_w2 + NW2 * W2_BYTES);
@@ -67,8 +61,6 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   uint64_t* s1_empty = s1_full + STAGES;
   uint64_t* w2_full = s1_empty + STAGES;
   uint64_t* w2_empty = w2_full + NW2;
-  uint64_t* ra_full = w2_empty + NW2;                                // [9] resident tap tiles
-  uint64_t* ra_empty = ra_full + 9;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_img = fp.tiles_x * fp.tiles_y;
@@ -81,7 +73,6 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     tma_prefetch_desc(&tma_a); tma_prefetch_desc(&tma_w1); tma_prefetch_desc(&tma_w2);
     for (int i = 0; i < STAGES; ++i) { mbar_init(&s1_full[i], 1); mbar_init(&s1_empty[i], EPI_WARPS); }
     for (int i = 0; i < NW2; ++i) { mbar_init(&w2_full[i], 1); mbar_init(&w2_empty[i], EPI_WARPS); }
-    for (int i = 0; i < 9; ++i) { mbar_init(&ra_full[i], 1); mbar_init(&ra_empty[i], EPI_WARPS); }
     mbar_fence_init();
   }
   for (int i = threadIdx.x; i < fp.Cmid; i += blockDim.x) s_b1[i] = fp.bias1 ? fp.bias1[i] : 0.f;
@@ -98,7 +89,7 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      int s = 0; uint32_t ph = 0; int wb = 0; uint32_t wph = 0; uint32_t raph = 0;
+      int s = 0; uint32_t ph = 0; int wb = 0; uint32_t wph = 0;
       auto load_w2 = [&](int j) {
         mbar_wait(&w2_empty[wb], wph ^ 1);
         mbar_expect_tx(&w2_full[wb], W2_BYTES);
@@ -111,21 +102,6 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         coords(tile, img, oy0, ox0);
         const int x0 = ox0 * fp.stride - 1, y0 = oy0 * fp.stride - 1;
         for (int j = 0; j < nch; ++j) {
-          if constexpr (RES_A) {
-            for (int pr = 0; pr < 5; ++pr) {                          // tap pairs (0,1) (2,3) (4,5) (6,7) (8,-)
-              if (j == 0) {
-                for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) {
-                  mbar_wait(&ra_empty[t], raph ^ 1);
-                  mbar_expect_tx(&ra_full[t], A1_BYTES);
-                  tma_load_4d(s_ra + t * A1_BYTES, &tma_a, &ra_full[t], 0, x0 + t % 3, y0 + t / 3, img);
-                }
-              }
-              mbar_wait(&s1_empty[s], ph ^ 1);
-              mbar_expect_tx(&s1_full[s], W1_BYTES);
-              tma_load_2d(s_1 + s * S1_BYTES, &tma_w1, &s1_full[s], pr * 64, j * CH);   // columns >= 288 are zero filled
-              if (++s == STAGES) { s = 0; ph ^= 1; }
-            }
-          } else {
           int kcol = 0;
           for (int r = 0; r < 3; ++r)
             for (int sx = 0; sx < 3; ++sx)
@@ -137,10 +113,8 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                 tma_load_2d(sa + A1_BYTES, &tma_w1, &s1_full[s], kcol, j * CH);
                 if (++s == STAGES) { s = 0; ph ^= 1; }
               }
-          }
           load_w2(j);
         }
-        raph ^= 1;
       }
     }
   } else if (warp >= 4) {
@@ -148,7 +122,7 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
     const int wg = (warp - 4) >> 2, ww = warp & 3;
     const int r0 = ww * 16 + (lane >> 2), c = (lane & 3) * 2;        // fragment rows r0, r0 + 8 (of the warpgroup), columns 8j + c
     uint8_t* a2 = s_a2 + wg * A2_WG_BYTES;
-    int s = 0; uint32_t ph = 0; int wb = 0; uint32_t wph = 0; uint32_t raph = 0;
+    int s = 0; uint32_t ph = 0; int wb = 0; uint32_t wph = 0;
     constexpr int NCH = 64;                                          // partial-sum width (register budget: d1 + d2 + part)
     float d1[CH / 2], d2[COUT / 2], part[NCH / 2];
     T* out = reinterpret_cast<T*>(fp.out);
@@ -161,37 +135,9 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
       int img, oy0, ox0;
       coords(tile, img, oy0, ox0);
       for (int j = 0; j < nch; ++j) {
-        // GEMM1: expanded chunk j
-        // (per-k-block partial sums added in fp32, gemm_epilogue.cuh: one k-block = one tap here, as in conv_igemm with BKC = 32)
-        if constexpr (RES_A) {
-#pragma unroll
-          for (int i = 0; i < CH / 2; ++i) d1[i] = 0.f;
-          for (int pr = 0; pr < 5; ++pr) {
-            mbar_wait(&s1_full[s], ph);
-            if (j == 0)
-              for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) mbar_wait(&ra_full[t], raph);
-            const uint64_t dbp = wgmma_desc_k128(smem_u32(s_1 + s * S1_BYTES));     // [128 x 64]: taps 2pr (cols 0..31), 2pr+1 (32..63)
-            for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) {
-              const uint64_t da = wgmma_desc_k64(smem_u32(s_ra + t * A1_BYTES) + wg * 64 * 64);
-#pragma unroll
-              for (int cn = 0; cn < CH / NCH; ++cn) {
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < 2; ++k)
-                  wgmma_m64k16<T, NCH>(part, da + 2 * k, dbp + ((cn * NCH * 128) >> 4) + 4 * (t & 1) + 2 * k, k != 0 ? 1u : 0u);
-                wgmma_commit();
-                wg_promote<NCH>(d1 + cn * (NCH / 2), part);
-              }
-            }
-            release(&s1_empty[s]);
-            if (j == nch - 1)
-              for (int t = 2 * pr; t < 2 * pr + 2 && t < 9; ++t) release(&ra_empty[t]);
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-          }
-        } else {
-          wg_mainloop<T, CH, BKC, NCH>(d1, s_1, S1_BYTES, A1_BYTES, STAGES, s1_full, s1_empty, s, ph, kb1, wg, lane,
-                                       [](const uint8_t*) {});
-        }
+        // GEMM1: expanded chunk j (per-k-block partial sums added in fp32, gemm_epilogue.cuh)
+        wg_mainloop<T, CH, BKC, NCH>(d1, s_1, S1_BYTES, A1_BYTES, STAGES, s1_full, s1_empty, s, ph, kb1, wg, lane,
+                                     [](const uint8_t*) {});
         // epi1: + shift -> round -> Hardswish -> round -> A2 (row r, mid channel cc: k-block cc / 64, 16-byte chunk (cc % 64) / 8)
         const float* bs = s_b1 + j * CH;
 #pragma unroll
@@ -229,7 +175,6 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         release(&w2_empty[wb]);                                      // A2 and the W2 buffer are free again
         if (++wb == NW2) { wb = 0; wph ^= 1; }
       }
-      raph ^= 1;
       // epi2: + shift (+ block input) -> round -> NHWC store
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -254,22 +199,18 @@ fmb_fused_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
 
 bool fmb_fused_ok(int Cin, int Cmid, int Cout, int ksize, int stride, int pad, int act1, int act2) {
   static int en = -1;
-  if (en < 0) { const char* e = getenv("SB_FMB_FUSED"); en = e ? (e[0] - '0') : 1; }
+  if (en < 0) { const char* e = getenv("SB_FMB_FUSED"); en = (e && e[0] == '0') ? 0 : 1; }
   if (!en) return false;
   if (ksize != 3 || pad != 1 || (stride != 1 && stride != 2) || act1 != ACT_HARDSWISH || act2 != ACT_NONE) return false;
-  // Cin = 32 (stage 0, block 0) is instantiated and tested against the two separate kernels, but stays opt-in (SB_FMB_FUSED=2):
-  // its speed against them has not been measured on H100
-  if (Cin == 32 && en < 2) return false;
-  if (Cin != 32 && Cin != 64 && Cin != 128) return false;
+  if (Cin != 64 && Cin != 128) return false;
   if (Cmid % 128 || Cmid < 128 || Cmid > 1024) return false;
   return Cout == 64 || Cout == 128;
 }
 
 template <typename T, int BKC, int COUT, int STAGES, int NW2>
 static int launch_fmb(int dtype, const void* in, const void* w1, const void* w2, const FmbParams& fp, cudaStream_t st) {
-  constexpr bool RES_A = (BKC == 32);
-  constexpr size_t S1 = RES_A ? static_cast<size_t>(128 * 64 * 2) : static_cast<size_t>(128 * BKC * 2) * 2;
-  const size_t SMEM = (RES_A ? 9 * 128 * 32 * 2 : 0) + STAGES * S1 + 32768 + NW2 * (COUT * 256) + (fp.Cmid + COUT) * 4 + 512 + 1024;
+  constexpr size_t S1 = static_cast<size_t>(128 * BKC * 2) * 2;
+  const size_t SMEM = STAGES * S1 + 32768 + NW2 * (COUT * 256) + (fp.Cmid + COUT) * 4 + 512 + 1024;
   auto kern = fmb_fused_kernel<T, BKC, COUT, STAGES, NW2>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM) != cudaSuccess) {
     cudaGetLastError();
@@ -279,8 +220,7 @@ static int launch_fmb(int dtype, const void* in, const void* w1, const void* w2,
   CUtensorMap ma, m1, m2;
   int rc = make_tma_nhwc(&ma, dtype, in, fp.n_img, fp.H, fp.W, fp.Cin, BKC, 16, 8, fp.stride, BKC * 2);
   if (rc) return rc;
-  rc = RES_A ? make_tma_2d(&m1, dtype, w1, fp.Cmid, 9 * fp.Cin, 9 * fp.Cin, 128)      // [128 x 64] boxes over tap pairs, 128B swizzle
-             : make_tma_2d_sw(&m1, dtype, w1, fp.Cmid, 9 * fp.Cin, 9 * fp.Cin, BKC, 128, BKC * 2);
+  rc = make_tma_2d_sw(&m1, dtype, w1, fp.Cmid, 9 * fp.Cin, 9 * fp.Cin, BKC, 128, BKC * 2);
   if (rc) return rc;
   rc = make_tma_2d(&m2, dtype, w2, COUT, fp.Cmid, fp.Cmid, COUT);
   if (rc) return rc;
@@ -303,8 +243,6 @@ int fmb_fused(int dtype, const void* in, const void* w1, const float* bias1, con
   fp.bias1 = bias1; fp.bias2 = bias2; fp.residual = residual; fp.out = out;
 #define FMB(T_) \
   do { \
-    if (Cin == 32 && Cout == 64) return launch_fmb<T_, 32, 64, 3, 2>(dtype, in, w1, w2, fp, st); \
-    if (Cin == 32 && Cout == 128) return launch_fmb<T_, 32, 128, 3, 1>(dtype, in, w1, w2, fp, st); \
     if (Cout == 64) return launch_fmb<T_, 64, 64, 3, 2>(dtype, in, w1, w2, fp, st); \
     return launch_fmb<T_, 64, 128, 3, 1>(dtype, in, w1, w2, fp, st); \
   } while (0)

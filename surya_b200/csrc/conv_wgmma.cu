@@ -13,9 +13,6 @@
 #include "ops.cuh"
 #include "sb_ptx.cuh"
 
-#include <cstdio>
-#include <cstdlib>
-
 namespace sb {
 
 int make_tma_2d_sw(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_k, int box_rows,
@@ -128,12 +125,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
       wg_acc_store<BN / 8>(d, 0, acc_s + wg * 64 * BN, BN, warp & 3, lane);
       asm volatile("bar.sync 1, 256;" ::: "memory");
       if (v2) {
-        epilogue_tile_v2<T, BN>(acc, p, stage, sbias, lane, half,
-                                [&](int r) {
-                                  const int mm = q * 32 + r;
-                                  const int yy = oy0 + mm / TW, xx = ox0 + mm % TW;
-                                  return (yy < cp.Ho && xx < cp.Wo) ? (img * cp.Ho + yy) * cp.Wo + xx : -1;
-                                }, nb * BN);
+        epilogue_tile_rt<T>(acc, p, stage, sbias, lane, half,
+                            [&](int r) {
+                              const int mm = q * 32 + r;
+                              const int yy = oy0 + mm / TW, xx = ox0 + mm % TW;
+                              return (yy < cp.Ho && xx < cp.Wo) ? (img * cp.Ho + yy) * cp.Wo + xx : -1;
+                            }, nb * BN, 1.0f, BN / 32);
       } else if (half == 0) {
         const int m = q * 32 + lane;
         const int oy = oy0 + m / TW, ox = ox0 + m % TW;
@@ -177,7 +174,7 @@ static int launch_conv(const ConvArgs& a, cudaStream_t stream) {
   ConvKParams cp{};
   cp.g.M = a.n_img * Ho * Wo; cp.g.N = a.Cout; cp.g.K = a.ksize * a.ksize * a.Cin;
   cp.g.C = a.out; cp.g.ldc = a.Cout; cp.g.bias = a.bias; cp.g.residual = a.residual; cp.g.ldr = a.Cout;
-  cp.g.act = a.act; cp.g.swiglu = 0; cp.g.out_f32 = 0; cp.g.group_m = 8; cp.g.group_k = 0; cp.g.dbg = nullptr; cp.g.w_constant = 0;
+  cp.g.act = a.act; cp.g.swiglu = 0; cp.g.out_f32 = 0; cp.g.group_m = 8; cp.g.group_k = 0; cp.g.w_constant = 0;
   cp.n_img = a.n_img; cp.Ho = Ho; cp.Wo = Wo; cp.Cin = a.Cin; cp.ksize = a.ksize; cp.stride = a.stride; cp.pad = a.pad;
   cp.tiles_x = (Wo + 15) / 16; cp.tiles_y = (Ho + 7) / 8;
   const int tiles = a.n_img * cp.tiles_x * cp.tiles_y * ((a.Cout + BN - 1) / BN);
@@ -196,14 +193,7 @@ static int launch_conv(const ConvArgs& a, cudaStream_t stream) {
 // wide: core matrix = 8 pixels x 16 B contiguous, SBO = one halo row (10 px x 16 B), LBO = one plane.  A tap (ty, tx) is then
 // nothing but a start-address offset of (ty * 10 + tx) * 16 bytes in the A descriptor (and the second consumer warpgroup's 64
 // rows start 8 halo rows further).  Per tile: 1 TMA box (180 lines), 23 KB of LDS + STS, 18 MMAs per warpgroup.  Weights
-// (9 x 32 x 32, 64B-swizzled) are loaded once per CTA.  Stride 1, pad 1.  SB_CONV_DBG=1 prints the timeline of CTA 0.
-#define HALO_STAMP(k_)                                                                                          \
-  do {                                                                                                          \
-    if (p.dbg && blockIdx.x == 0) {                                                                             \
-      const int ti_ = (tile - blockIdx.x) / gridDim.x;                                                          \
-      if (ti_ < 48) p.dbg[ti_ * 8 + (k_)] = clock64();                                                          \
-    }                                                                                                           \
-  } while (0)
+// (9 x 32 x 32, 64B-swizzled) are loaded once per CTA.  Stride 1, pad 1.
 constexpr int HALO_BUFS = 8;       // halo boxes in flight (TMA staging, pixel-major)
 constexpr int HALO_PLANES = 3;     // re-laid tiles between the builders and the MMA warp
 constexpr int HALO_PLANE_PITCH = 180 * 16 + 32;   // +32: the four planes start in different bank groups (conflict-free STS)
@@ -262,7 +252,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tma_halo, const __grid_cons
         mbar_wait(&hempty_bar[hb], hph ^ 1);
         mbar_expect_tx(&hfull_bar[hb], HALO_BYTES);
         tma_load_4d(s_halo + hb * HALO_BYTES, &tma_halo, &hfull_bar[hb], 0, ox0 - 1, oy0 - 1, img);
-        HALO_STAMP(0);
         if (++hb == HALO_BUFS) { hb = 0; hph ^= 1; }
       }
     }
@@ -274,7 +263,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tma_halo, const __grid_cons
     int pb = 0; uint32_t pph = 0; int hb = 0; uint32_t hph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       mbar_wait(&hfull_bar[hb], hph);
-      if (i == 0) { HALO_STAMP(1); }
       const uint8_t* halo = s_halo + hb * HALO_BYTES;
       mbar_wait(&pempty_bar[pb], pph ^ 1);
       uint8_t* pl = s_pl + pb * PLANES_BYTES + c * HALO_PLANE_PITCH;
@@ -292,7 +280,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tma_halo, const __grid_cons
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) { mbar_arrive(&pfull_bar[pb]); mbar_arrive(&hempty_bar[hb]); }
-      if (i == 0) { HALO_STAMP(2); }
       if (++pb == HALO_PLANES) { pb = 0; pph ^= 1; }
       if (++hb == HALO_BUFS) { hb = 0; hph ^= 1; }
     }
@@ -306,19 +293,14 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tma_halo, const __grid_cons
     float* sbias = reinterpret_cast<float*>(epi_smem + EPI_WARPS * EPI_STAGE_BYTES);
     const uint32_t lbo = static_cast<uint32_t>(cp.desc_lbo), sbo = static_cast<uint32_t>(cp.desc_sbo);
     int pb = 0; uint32_t pph = 0;
-    const bool vec_ok = (p.ldc % 8 == 0) && (!p.residual || p.ldr % 8 == 0);
-    const bool v2 = epilogue_v2_ok(p);
     const AccRow acc(acc_s, q * 32 + lane, BN);
     float d[BN / 2];
-    if (v2) {
-      epilogue_stage_bias<BN>(p, sbias, epi_tid, 0);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
+    epilogue_stage_bias<BN>(p, sbias, epi_tid, 0);
+    asm volatile("bar.sync 1, 256;" ::: "memory");
     mbar_wait(w_bar, 0);
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int img, oy0, ox0;
       coords(tile, img, oy0, ox0);
-      if (epi_tid == 0) { HALO_STAMP(3); }
       mbar_wait(&pfull_bar[pb], pph);
       const uint32_t a0 = smem_u32(s_pl + pb * PLANES_BYTES) + wg * (TH / 2) * HW_ * 16;   // this warpgroup's 8 pixel rows
 #pragma unroll
@@ -341,37 +323,23 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tma_halo, const __grid_cons
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&pempty_bar[pb]);
-      if (epi_tid == 0) { HALO_STAMP(4); }
       if (++pb == HALO_PLANES) { pb = 0; pph ^= 1; }
       asm volatile("bar.sync 1, 256;" ::: "memory");   // the accumulator tile is free
       wg_acc_store<BN / 8>(d, 0, acc_s + wg * 64 * BN, BN, warp & 3, lane);
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (epi_tid == 0) { HALO_STAMP(5); }
-      if (v2) {
-        epilogue_tile_v2<T, BN>(acc, p, stage, sbias, lane, half,
-                                [&](int r) {
-                                  const int mm = q * 32 + r;
-                                  const int yy = oy0 + mm / TW, xx = ox0 + mm % TW;
-                                  return (yy < cp.Ho && xx < cp.Wo) ? (img * cp.Ho + yy) * cp.Wo + xx : -1;
-                                }, 0);
-      } else if (half == 0) {
-        const int m = q * 32 + lane;
-        const int oy = oy0 + m / TW, ox = ox0 + m % TW;
-        const bool row_ok = oy < cp.Ho && ox < cp.Wo;
-        const int row = (img * cp.Ho + oy) * cp.Wo + ox;
-        uint32_t v[32];
-        acc.load32(0, v);
-        epilogue_chunk<T>(v, p, row, row_ok, 0, vec_ok);
-      }
-      if (epi_tid == 0) { HALO_STAMP(6); }
+      // Cout = ldc = ldr = 32 and 16-bit output: the staged epilogue's requirements (epilogue_v2_ok) always hold here
+      epilogue_tile_rt<T>(acc, p, stage, sbias, lane, half,
+                          [&](int r) {
+                            const int mm = q * 32 + r;
+                            const int yy = oy0 + mm / TW, xx = ox0 + mm % TW;
+                            return (yy < cp.Ho && xx < cp.Wo) ? (img * cp.Ho + yy) * cp.Wo + xx : -1;
+                          }, 0, 1.0f, BN / 32);
     }
   }
 }
 
 static bool conv_halo_ok(const ConvArgs& a) {
-  static int en = -1;
-  if (en < 0) { const char* e = getenv("SB_CONV_HALO"); en = (e && e[0] == '0') ? 0 : 1; }
-  return en && a.ksize == 3 && a.stride == 1 && a.pad == 1 && a.Cin == 32 && a.Cout == 32;
+  return a.ksize == 3 && a.stride == 1 && a.pad == 1 && a.Cin == 32 && a.Cout == 32;
 }
 
 template <typename T>
@@ -396,33 +364,12 @@ static int launch_conv_halo(const ConvArgs& a, cudaStream_t stream) {
   ConvKParams cp{};
   cp.g.M = a.n_img * a.H * a.W; cp.g.N = a.Cout; cp.g.K = 9 * a.Cin;
   cp.g.C = a.out; cp.g.ldc = a.Cout; cp.g.bias = a.bias; cp.g.residual = a.residual; cp.g.ldr = a.Cout;
-  cp.g.act = a.act; cp.g.swiglu = 0; cp.g.out_f32 = 0; cp.g.group_m = 8; cp.g.group_k = 0; cp.g.dbg = nullptr; cp.g.w_constant = 0;
+  cp.g.act = a.act; cp.g.swiglu = 0; cp.g.out_f32 = 0; cp.g.group_m = 8; cp.g.group_k = 0; cp.g.w_constant = 0;
   cp.n_img = a.n_img; cp.Ho = a.H; cp.Wo = a.W; cp.Cin = a.Cin; cp.ksize = 3; cp.stride = 1; cp.pad = 1;
   cp.tiles_x = (a.W + 7) / 8; cp.tiles_y = (a.H + 15) / 16;
   cp.desc_lbo = HALO_PLANE_PITCH; cp.desc_sbo = 10 * 16;   // LBO: next 16-byte k chunk (plane); SBO: next 8-row group (halo row)
   const int tiles = a.n_img * cp.tiles_x * cp.tiles_y;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  static int dbg_on = -1;
-  if (dbg_on < 0) { const char* e = getenv("SB_CONV_DBG"); dbg_on = (e && e[0] == '1') ? 1 : 0; }
-  if (dbg_on) {
-    unsigned long long* d = nullptr;
-    cudaMalloc(&d, 48 * 8 * 8);
-    cudaMemset(d, 0, 48 * 8 * 8);
-    cp.g.dbg = reinterpret_cast<decltype(cp.g.dbg)>(d);
-    kern<<<grid, 512, SMEM, stream>>>(mh, mb, cp);
-    cudaStreamSynchronize(stream);
-    unsigned long long h[48 * 8];
-    cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    fprintf(stderr, "conv_halo timeline (CTA 0, cycles since first stamp): tile | tma issued | halo landed | built | mma start | mma done | epi start | epi done\n");
-    for (int t = 0; t < 48; ++t) {
-      fprintf(stderr, "%3d", t);
-      for (int k = 0; k < 7; ++k) fprintf(stderr, " %8lld", h[t * 8 + k] ? (long long)(h[t * 8 + k] - h[0]) : -1LL);
-      fprintf(stderr, "\n");
-    }
-    dbg_on = 0;
-    return launch_ok();
-  }
   kern<<<grid, 512, SMEM, stream>>>(mh, mb, cp);
   return launch_ok();
 }

@@ -32,7 +32,6 @@ struct GemmArgs {
   int group_k = 0, group_n = 0, a_cols = 0;
   int w_constant = 0;                     // W is never written by a preceding kernel: its tiles may be prefetched
                                           // before the programmatic-dependency wait (engine weights)
-  unsigned long long* dbg = nullptr;      // optional in-kernel timeline (see GemmKParams::dbg)
   // RMSNorm folded into the GEMM: C = epi(rs[m] * (A W^T) + bias), W already multiplied by the norm weight.
   //   rowscale  : rs given, fp32 [M] (row_rstd in ops.cu)
   //   ssq_inline: rs = rsqrt(sum_k A[m,k]^2 / ssq_k + ssq_eps) computed inside the kernel from the A tiles
@@ -50,10 +49,6 @@ struct GemmArgs {
 // M <= 16 rows: mma.sync kernel without the wgmma pipeline set-up costs (gemm_skinny.cu); gemm_launch routes to it when it applies.
 bool gemm_skinny_ok(const GemmArgs& a);
 int gemm_skinny_launch(const GemmArgs& a, cudaStream_t stream);
-// Several dependent skinny GEMMs in one persistent launch with grid-wide barriers between them (gemm_chain.cu); `bar` = 3
-// zero-initialised uint32 owned by the caller (re-armed by the kernel).  phases[i].force_bn > 0 fixes that phase's tile width.
-int gemm_chain_launch(const GemmArgs* phases, int n, unsigned int* bar, cudaStream_t stream);
-int gemm_chain_bn(int M, int N, int swiglu);
 // Tile width gemm_launch will use for an argmax-epilogue launch of this shape (partials per row = ceil(N / width)).
 int gemm_argmax_tile(int M, int N);
 
@@ -71,8 +66,7 @@ long long launch_count();
 void count_launches(long long n);  // kernels replayed through a CUDA graph
 int num_sms();
 
-// Launch with the programmatic-stream-serialization attribute (PDL) unless SB_PDL=0.
-bool pdl_enabled();
+// Launch with the programmatic-stream-serialization attribute (PDL).
 template <typename... P, typename... A>
 inline cudaError_t launch_pdl(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A... args) {
   cudaLaunchConfig_t cfg = {};
@@ -81,7 +75,7 @@ inline cudaError_t launch_pdl(void (*kernel)(P...), dim3 grid, dim3 block, size_
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<P>(args)...);
 }
 

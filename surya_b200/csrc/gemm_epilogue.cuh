@@ -35,8 +35,6 @@ struct GemmKParams {
   float* am_sum;
   int am_ld;
   int store_c;
-  unsigned long long* dbg;  // optional timeline buffer (globaltimer ns) written by CTA 0: [0]=start [1]=setup done
-                            // [2+kb]=k-block kb landed (first tile) [40]=accumulator ready [41]=epilogue done
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -182,7 +180,7 @@ __device__ __forceinline__ void wg_acc_store(const float* d, int j0, float* dst,
 // Accumulation: the tensor core adds its products into the accumulator with truncation, so over a long K the error of a
 // single accumulator chain grows with K and is biased.  Each slot's MMAs therefore run into a fresh partial (NCH columns at a
 // time, NCH <= BN) that is then added to d in fp32 with round-to-nearest: d = ((0 + p_0) + p_1) + ...  Every kernel that
-// must agree bit for bit with another (fused vs unfused, chain vs separate launches, any tile width) sums this way, per
+// must agree bit for bit with another (fused vs unfused, any tile width) sums this way, per
 // k-block of the same K order.
 template <typename T, int BN, int BK, int NCH = (BN < ACC_MAX_COLS ? BN : ACC_MAX_COLS), typename StageFn>
 __device__ __forceinline__ void wg_mainloop(float* d, const uint8_t* ring, uint32_t slot_bytes, uint32_t a_bytes, int stages,
@@ -482,11 +480,6 @@ __device__ __forceinline__ void epilogue_stage_bias(const GemmKParams& p, float*
     sbias[j] = (p.bias && n_col0 + j < p.N) ? __ldg(p.bias + n_col0 + j) : 0.f;
 }
 
-__device__ __forceinline__ void epilogue_stage_bias_rt(const GemmKParams& p, float* sbias, int epi_tid, int n_col0, int bn) {
-  for (int j = epi_tid; j < bn; j += EPI_WARPS * 32)
-    sbias[j] = (p.bias && n_col0 + j < p.N) ? __ldg(p.bias + n_col0 + j) : 0.f;
-}
-
 // Runtime -> compile-time dispatch on (act, swiglu); once per tile, outside every loop.  ng = 32-column groups in the tile.
 template <typename T, typename RowFn>
 __device__ __forceinline__ void epilogue_tile_rt(const AccRow& acc, const GemmKParams& p, uint8_t* stage, const float* sbias,
@@ -504,12 +497,6 @@ __device__ __forceinline__ void epilogue_tile_rt(const AccRow& acc, const GemmKP
     case ACT_SILU: epilogue_tile_ct<T, ACT_SILU, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
     default: epilogue_tile_ct<T, ACT_GELU_TANH, false>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, ng); break;
   }
-}
-
-template <typename T, int BN, typename RowFn>
-__device__ __forceinline__ void epilogue_tile_v2(const AccRow& acc, const GemmKParams& p, uint8_t* stage, const float* sbias,
-                                                 int lane, int half, RowFn row_fn, int n_col0, float rs = 1.0f) {
-  epilogue_tile_rt<T>(acc, p, stage, sbias, lane, half, row_fn, n_col0, rs, BN / 32);
 }
 
 }  // namespace sb

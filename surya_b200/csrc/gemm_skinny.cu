@@ -15,8 +15,6 @@
 #include "gemm_epilogue.cuh"
 #include "sb_ptx.cuh"
 
-#include <cstdlib>
-
 namespace sb {
 
 struct SkinnyParams {
@@ -134,9 +132,6 @@ __global__ void __launch_bounds__(SK_WARPS * 32) gemm_skinny_kernel(const Skinny
 }
 
 bool gemm_skinny_ok(const GemmArgs& a) {
-  static int en = -1;
-  if (en < 0) { const char* e = getenv("SB_SKINNY"); en = (e && e[0] == '0') ? 0 : 1; }
-  if (!en) return false;
   if (a.M > 16 || a.M <= 0 || a.out_f32 || a.group_k || a.rowscale || a.ssq_inline || a.am_val || a.force_bn > 0) return false;
   if (a.K % 32 || a.lda % 8 || a.ldw % 8) return false;
   if ((reinterpret_cast<uintptr_t>(a.A) | reinterpret_cast<uintptr_t>(a.W)) & 15) return false;

@@ -251,7 +251,7 @@ static int launch_splitk(const GemmArgs& a, int pk, cudaStream_t stream) {
   p.bias = a.bias;
   p.residual = a.residual; p.ldr = a.ldr;
   p.act = a.act; p.swiglu = a.swiglu; p.out_f32 = 0;
-  p.group_m = 1; p.group_k = 0; p.dbg = nullptr;
+  p.group_m = 1; p.group_k = 0;
   p.w_constant = a.w_constant;
   const int m_blocks = (a.M + 127) / 128, n_blocks = (a.N + BN - 1) / BN;
   cudaLaunchConfig_t cfg = {};
@@ -265,7 +265,7 @@ static int launch_splitk(const GemmArgs& a, int pk, cudaStream_t stream) {
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
+  cfg.numAttrs = 2;
   cudaLaunchKernelEx(&cfg, kern, ma, mb, p, pk, rstride, stages);
   return launch_ok();
 }

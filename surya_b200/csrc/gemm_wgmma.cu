@@ -21,7 +21,6 @@
 #include "sb_ptx.cuh"
 
 #include <cstdarg>
-#include <cstdlib>
 #include <cstdio>
 #include <atomic>
 #include <mutex>
@@ -55,14 +54,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  auto stamp = [&](int slot) {
-    if (p.dbg && blockIdx.x == 0) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      p.dbg[slot] = t;
-    }
-  };
-  if (threadIdx.x == 0) stamp(0);
   pdl_trigger();
   const int m_blocks = (p.M + BM - 1) / BM;
   const int n_blocks = (p.N + BN - 1) / BN;
@@ -79,7 +70,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     mbar_fence_init();
   }
   __syncthreads();
-  if (threadIdx.x == 0) stamp(1);
 
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
@@ -145,19 +135,14 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       }
       // sum of squares of the tile's 128 A rows (folded RMSNorm), taken from each stage while its MMAs run
       float ssq = 0.f;
-      const bool first = tile == static_cast<int>(blockIdx.x);
-      int kb_seen = 0;
       wg_mainloop<T, BN, BK>(d, smem, STAGE_BYTES, A_BYTES, STAGES, full_bar, empty_bar, s, ph, k_blocks, wg, lane,
                              [&](const uint8_t* slot) {
-                               if (first && epi_tid == 0 && kb_seen < 38) stamp(2 + kb_seen);
-                               ++kb_seen;
                                if (p.ssq_inline) ssq = ssq_stage<T>(slot, epi_tid, ssq);
                              });
       if (p.ssq_inline) {
         const float tot = ssq + __shfl_xor_sync(0xffffffffu, ssq, 1);
         if ((epi_tid & 1) == 0) srs[epi_tid >> 1] = rsqrtf(tot * p.ssq_inv_k + p.ssq_eps);
       }
-      if (epi_tid == 0 && first) stamp(40);
       const int row0 = mb * BM + q * 32;
 #pragma unroll
       for (int c0 = 0; c0 < BN; c0 += AC) {
@@ -187,10 +172,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           }
         }
       }
-      if (epi_tid == 0 && first) stamp(41);
     }
   }
-  if (threadIdx.x == 0) stamp(42);
 }
 
 // ----------------------------------------------------------------------------------- host side
@@ -205,16 +188,6 @@ const char* last_error() { return g_err; }
 
 static std::atomic<long long> g_launches{0};
 long long launch_count() { return g_launches.load(); }
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("SB_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
-bool splitk_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("SB_SPLITK"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
 void count_launches(long long n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int launch_ok() {
   g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -386,7 +359,6 @@ static int launch_cfg(const GemmArgs& a, cudaStream_t stream) {
   p.act = a.act; p.swiglu = a.swiglu; p.out_f32 = a.out_f32;
   p.group_m = 8;
   p.group_k = a.group_k;
-  p.dbg = a.dbg;
   p.w_constant = a.w_constant;
   p.rowscale = a.rowscale;
   p.ssq_inline = a.ssq_inline;
@@ -404,7 +376,7 @@ template <typename T>
 static int launch_typed(const GemmArgs& a, cudaStream_t stream) {
   int bn = a.force_bn;
   if (bn >= 1000) return gemm_splitk_launch(a, bn / 1000, bn % 1000, stream);   // forced split-K: 1000 * pk + BN
-  if (bn == 0 && a.allow_splitk && splitk_enabled() && !a.rowscale && !a.ssq_inline && !a.am_val) {
+  if (bn == 0 && a.allow_splitk && !a.rowscale && !a.ssq_inline && !a.am_val) {
     int sbn = 0;
     const int pk = splitk_plan(a, &sbn);
     if (pk >= 2) return gemm_splitk_launch(a, pk, sbn, stream);

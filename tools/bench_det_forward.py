@@ -1,5 +1,5 @@
 """Detection forward only (GPU box): BASELINE config 3 (32 pages 1024^2, fp16) resident forward, CUDA-event timed; prints ms
-per forward and pages/s.  Environment switches of the kernels under test are read by the library (SB_DET_FUSED_HEAD, SB_CONV_HALO)."""
+per forward and pages/s.  Environment switches of the kernels under test are read by the library (SB_DET_FUSED_HEAD, SB_FMB_FUSED)."""
 import sys
 from pathlib import Path
 
