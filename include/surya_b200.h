@@ -42,7 +42,11 @@ long long sb_launch_count(void);
  * C[M,Nout] = epi(A[M,K] @ W[N,K]^T).  bias is fp32 [N] or NULL; residual [M,Nout] or NULL.
  * swiglu=1: W rows interleaved (gate_i, up_i), Nout = N/2, out = act(gate)*up.  out_f32: C is float32.
  * force_bn: 0 = tile heuristic; 32/64/96/128/256 = fixed tile width; -1 = heuristic that may also pick the split-K cluster
- * kernel (fp32 partials summed in a fixed order over <= 3 K slices; for decode-sized M <= 256 callers); 1000*pk + BN forces it. */
+ * kernel (fp32 partials summed in a fixed order over <= 3 K slices; for decode-sized M <= 256 callers); 1000*pk + BN forces it.
+ * Rejected with a negative code (see sb_last_error): A, W, C or residual not 16-byte aligned, an lda / ldw pitch that is not
+ * a multiple of 16 bytes, swiglu with a residual, out_f32 with a residual or with swiglu.  C may be the residual (in place).
+ * Preceding kernels on the stream may still be running when this one starts (programmatic dependent launch); A, W, bias and
+ * residual are read only after they have completed. */
 int sb_gemm(int dtype, const void* A, int lda, const void* W, int ldw, void* C, int ldc, int M, int N, int K,
             const float* bias, const void* residual, int ldr, int act, int swiglu, int out_f32, int force_bn,
             void* stream);

@@ -25,6 +25,7 @@ struct SkinnyParams {
   const float* bias;
   const void* residual; int ldr;
   int act, swiglu;
+  int w_constant;   // W is never written by a preceding kernel: its first loads may precede the dependency wait
 };
 
 template <typename T> struct MmaSkinny;
@@ -63,13 +64,15 @@ __global__ void __launch_bounds__(SK_WARPS * 32) gemm_skinny_kernel(const Skinny
   const T* A1 = reinterpret_cast<const T*>(p.A) + static_cast<size_t>(r + 8 < p.M ? r + 8 : 0) * p.lda + q * 8;
   const bool a0_ok = r < p.M, a1_ok = r + 8 < p.M;
   float c[4] = {0.f, 0.f, 0.f, 0.f};
-  // weights never depend on the previous kernel: the first batch of W loads goes out before the dependency wait
+  // constant weights (w_constant) do not depend on the previous kernel: their first batch of loads goes out before the
+  // dependency wait.  Any other W may still be being written by the previous kernel, so it is read after the wait.
+  if (!p.w_constant) pdl_wait();
   uint4 w[SK_UNROLL];
   int kb = kb0;
 #pragma unroll
   for (int u = 0; u < SK_UNROLL; ++u)
     w[u] = (n_ok && kb + u < kb1) ? *reinterpret_cast<const uint4*>(Wrow + static_cast<size_t>(kb + u) * 32) : make_uint4(0u, 0u, 0u, 0u);
-  pdl_wait();
+  if (p.w_constant) pdl_wait();
   for (; kb < kb1; kb += SK_UNROLL) {
     uint4 a0[SK_UNROLL], a1[SK_UNROLL];
 #pragma unroll
@@ -143,6 +146,7 @@ int gemm_skinny_launch(const GemmArgs& a, cudaStream_t stream) {
   SkinnyParams p;
   p.A = a.A; p.lda = a.lda; p.W = a.W; p.ldw = a.ldw; p.C = a.C; p.ldc = a.ldc;
   p.M = a.M; p.N = a.N; p.K = a.K; p.bias = a.bias; p.residual = a.residual; p.ldr = a.ldr; p.act = a.act; p.swiglu = a.swiglu;
+  p.w_constant = a.w_constant;
   const dim3 grid((a.N + 7) / 8), block(SK_WARPS * 32);
   if (a.dtype == DT_BF16) launch_pdl(gemm_skinny_kernel<__nv_bfloat16>, grid, block, 0, stream, p);
   else launch_pdl(gemm_skinny_kernel<__half>, grid, block, 0, stream, p);

@@ -428,6 +428,18 @@ int gemm_argmax_tile(int M, int N) {
 
 int gemm_launch(const GemmArgs& a, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return 0;
+  // Every epilogue may store C and load the residual in 16-byte vectors, and none of them combines these options; the
+  // arguments are rejected here rather than faulting the device or being dropped silently on one path.
+  if ((reinterpret_cast<uintptr_t>(a.C) & 15) != 0) {
+    set_error("gemm: C must be 16B aligned (ptr=%p)", a.C);
+    return -19;
+  }
+  if ((reinterpret_cast<uintptr_t>(a.residual) & 15) != 0) {
+    set_error("gemm: the residual must be 16B aligned (ptr=%p)", a.residual);
+    return -19;
+  }
+  if (a.swiglu && a.residual) { set_error("gemm: the swiglu epilogue takes no residual"); return -20; }
+  if (a.out_f32 && (a.residual || a.swiglu)) { set_error("gemm: out_f32 takes no residual and no swiglu"); return -20; }
   if (a.rowscale || a.ssq_inline || a.am_val) {
     // these ride on the staged 16-bit epilogue only (and on the plain kernel: split-K would change who owns a row's columns)
     const bool v2 = !a.out_f32 && a.ldc % 8 == 0 && (!a.residual || a.ldr % 8 == 0) &&

@@ -50,7 +50,8 @@ def _act_ref(x, act):
     [
         (128, 256, 64, 256), (128, 128, 128, 128), (256, 64, 1280, 64), (200, 96, 592, 32),
         (1000, 1280, 592, 0), (640, 3840, 1280, 0), (256, 1280, 3456, 0), (333, 520, 1280, 128),
-        (4096, 1280, 1280, 256),
+        (4096, 1280, 1280, 256), (333, 520, 640, 96), (1153, 2560, 1280, 128), (130, 256, 8, 0), (200, 392, 40, 64),
+        (200, 100, 256, 64),
     ],
 )
 def test_gemm_plain(built_lib, dtype, M, N, K, bn):
@@ -66,17 +67,30 @@ def test_gemm_plain(built_lib, dtype, M, N, K, bn):
 
 
 @pytest.mark.parametrize("dtype", DT)
-@pytest.mark.parametrize("act", ["none", "gelu", "silu", "hardswish", "relu", "gelu_tanh"])
-def test_gemm_epilogue(built_lib, dtype, act):
+@pytest.mark.parametrize("act,bn,swiglu", [
+    *[pytest.param(act, 0, False, id=act) for act in ["none", "gelu", "silu", "hardswish", "relu", "gelu_tanh"]],
+    # the 256-wide tile's two-pass epilogue with a residual and with SwiGLU; SwiGLU with gelu_erf (the epilogue_chunk fallback)
+    pytest.param("gelu", 256, False, id="gelu-bn256"),
+    pytest.param("silu", 256, True, id="swiglu-silu-bn256"),
+    pytest.param("gelu", 0, True, id="swiglu-gelu_erf"),
+])
+def test_gemm_epilogue(built_lib, dtype, act, bn, swiglu):
     from surya_b200 import ops
 
-    M, N, K = 300, 392, 320
+    M, N, K = 300, 400 if swiglu else 392, 320
     g = torch.Generator(device="cuda").manual_seed(11)
     a = (torch.randn(M, K, device="cuda", generator=g)).to(dtype)
     w = (torch.randn(N, K, device="cuda", generator=g) * 0.08).to(dtype)
     bias = torch.randn(N, device="cuda", generator=g).to(dtype).float()
+    if swiglu:   # SwiGLU takes no residual; W rows interleave (gate_i, up_i)
+        out = ops.gemm(a, w, bias=bias, act=act, swiglu=True, force_bn=bn)
+        torch.cuda.synchronize()
+        lin = (a.float() @ w.float().t() + bias).to(dtype).float()
+        ref = (_act_ref(lin[:, 0::2], act).to(dtype).float() * lin[:, 1::2]).to(dtype)
+        _close(out, ref, dtype, ulps=3.0, what=f"gemm swiglu epilogue {act} bn={bn}")
+        return
     res = torch.randn(M, N, device="cuda", generator=g).to(dtype)
-    out = ops.gemm(a, w, bias=bias, residual=res, act=act)
+    out = ops.gemm(a, w, bias=bias, residual=res, act=act, force_bn=bn)
     torch.cuda.synchronize()
     lin = (a.float() @ w.float().t() + bias).to(dtype)
     y = _act_ref(lin.float(), act).to(dtype) if act != "none" else lin
@@ -429,6 +443,7 @@ def test_embed_splice_and_heads(built_lib, dtype):
         (256, 1280, 1280, 2, 64, "none"), (256, 1280, 1280, 3, 64, "bias_res_gelu"), (16, 1024, 1024, 8, 128, "none"),
         (130, 1000, 640, 5, 128, "bias"), (256, 512, 1280, 8, 64, "swiglu"), (96, 4096, 1024, 2, 128, "geglu"),
         (256, 1280, 1280, 0, 0, "res"), (256, 1920, 1280, 0, 0, "bias"), (16, 512, 1024, 0, 0, "none"),
+        (256, 1280, 192, 2, 64, "res"),
     ],
 )
 def test_gemm_splitk_cluster(built_lib, dtype, M, N, K, pk, bn, epi):
@@ -466,7 +481,8 @@ def test_gemm_splitk_cluster(built_lib, dtype, M, N, K, pk, bn, epi):
 # ------------------------------------------------------------------------------------------------ error behaviour
 def test_errors_are_loud(built_lib):
     """Bad arguments come back as a negative code + message through the C ABI (raised as SuryaB200Error), never as a silent
-    fallback: misaligned TMA pitch, odd SwiGLU width, unsupported head_dim / GQA group, unsupported depthwise kernel size."""
+    fallback: misaligned TMA pitch, odd SwiGLU width, unsupported head_dim / GQA group, unsupported depthwise kernel size,
+    misaligned C or residual, SwiGLU with a residual, fp32 output with a residual or with SwiGLU."""
     from surya_b200 import _lib, ops
 
     dt = torch.bfloat16
@@ -489,6 +505,22 @@ def test_errors_are_loud(built_lib):
     x = torch.randn(1, 8, 8, 16, device="cuda").half()
     with pytest.raises(_lib.SuryaB200Error, match="kernel size"):
         ops.dwconv_nhwc(x, torch.randn(49, 16, device="cuda").half(), None, 7, 1, 3, "none")
+    # C and the residual are stored / loaded in 16-byte vectors: a window 4 elements (8 bytes) into a buffer is refused
+    a = torch.randn(64, 128, device="cuda").to(dt)
+    w = torch.randn(32, 128, device="cuda").to(dt)
+    buf = torch.zeros(64, 48, device="cuda", dtype=dt)
+    with pytest.raises(_lib.SuryaB200Error, match="C must be 16B aligned"):
+        ops.gemm(a, w, out=buf[:, 4:36])
+    with pytest.raises(_lib.SuryaB200Error, match="residual must be 16B aligned"):
+        ops.gemm(a, w, residual=buf[:, 4:36])
+    # option combinations no epilogue implements
+    res = torch.randn(64, 16, device="cuda").to(dt)
+    with pytest.raises(_lib.SuryaB200Error, match="swiglu epilogue takes no residual"):
+        ops.gemm(a, w, act="silu", swiglu=True, residual=res)
+    with pytest.raises(_lib.SuryaB200Error, match="out_f32 takes no residual"):
+        ops.gemm(a, w, out_f32=True, residual=torch.randn(64, 32, device="cuda").to(dt))
+    with pytest.raises(_lib.SuryaB200Error, match="out_f32 takes no residual and no swiglu"):
+        ops.gemm(a, w, act="silu", swiglu=True, out_f32=True)
     # and the library keeps working after an error
     a = torch.randn(64, 128, device="cuda").to(dt)
     w = torch.randn(32, 128, device="cuda").to(dt)
@@ -499,7 +531,8 @@ def test_errors_are_loud(built_lib):
 
 @pytest.mark.parametrize("dtype", DT)
 @pytest.mark.parametrize("M,N,K,epi", [(16, 1024, 1024, "bias"), (16, 8192, 1024, "geglu"), (16, 1024, 4096, "res"), (3, 520, 320, "gelu"),
-                                       (16, 1536, 1024, "none"), (1, 20, 1024, "none")])
+                                       (16, 1536, 1024, "none"), (1, 20, 1024, "none"),
+                                       (16, 264, 512, "res"), (17, 264, 512, "res"), (8, 264, 40, "bias")])
 def test_gemm_skinny_path(built_lib, dtype, M, N, K, epi):
     """M <= 16 routes to the mma.sync kernel (gemm_skinny.cu): against the fp32 restatement with the output roundings, and
     against the wgmma kernel (forced tile width) to a few ulp — the two paths sum in different orders."""
