@@ -282,6 +282,31 @@ int sb_dwconv_nhwc(int dtype, const void* in, const void* w, const float* bias, 
                    int ks, int stride, int pad, int act, void* stream);
 int sb_gemm_grouped(int dtype, const void* A, int lda, int a_cols, const void* W, int ldw, void* C, int ldc, int M, int N,
                     int Kpad, int group_k, int group_n, void* stream);
+/* The engine's detection kernels one at a time (op-level entry points used by the kernel tests); arguments as the engine
+ * passes them (surya_b200/detection.py:pack_det_program for the weight layouts), outputs dense at the given pointer.
+ * Stem: NCHW [B,3,H,W] (engine dtype, or fp32 when in_f32), w fp32 [cout][3][3][3] (r, s, c), bias fp32 -> NHWC [B,H/2,W/2,cout]
+ * (cout = 32; H, W even). */
+int sb_det_stem_conv(int dtype, const void* in, int in_f32, const float* w, const float* bias, void* out, int B, int H, int W,
+                     int cout, void* stream);
+/* FusedMBConv: NHWC [n_img,H,W,Cin] -> 3x3 expand (w1 [Cmid][9*Cin], bias1 fp32) + Hardswish -> 1x1 project (w2 [Cout][Cmid],
+ * bias2 fp32) (+ residual NHWC [n_img,Ho,Wo,Cout], may be null) -> out NHWC [n_img,Ho,Wo,Cout].  Cin 64 / 128, Cmid a multiple
+ * of 128 up to 1024, Cout 64 / 128, stride 1 / 2. */
+int sb_det_fmb_fused(int dtype, const void* in, const void* w1, const float* bias1, const void* w2, const float* bias2,
+                     const void* residual, void* out, int n_img, int H, int W, int Cin, int Cmid, int Cout, int stride,
+                     void* stream);
+/* Decode head in one kernel: srcs[i] NHWC [B,hs[i],ws[i],CS] placed at channel ch_off[i] of the concat, bilinear up-sampled to
+ * HO x WO -> fuse_w [512][512] + fuse_bias fp32 + ReLU -> cls_w [2][512] + cls_b [2] -> sigmoid -> logits NCHW [B,2,HO,WO].
+ * Four sources of 128 channels, one of them HO x WO, the others at ratio 2, 4 or 8 in each direction. */
+int sb_det_head_fused(int dtype, const void* const* srcs, const int* hs, const int* ws, const int* ch_off, int n_src, int CS,
+                      const void* fuse_w, const float* fuse_bias, const void* cls_w, const void* cls_b, void* logits, int B,
+                      int HO, int WO, void* stream);
+/* Bilinear (align_corners=False) up-sampling of 1..4 NHWC maps [B,hs[i],ws[i],CS] to HO x WO, written at channel ch_off[i] of
+ * dst NHWC [B,HO,WO,n_src*CS] (CS % 8 == 0). */
+int sb_det_upsample_cat(int dtype, const void* const* srcs, const int* hs, const int* ws, const int* ch_off, int n_src, int CS,
+                        void* dst, int B, int HO, int WO, void* stream);
+/* x NHWC [P,C] (P = B*HW), w [n_out][C], b [n_out] -> out NCHW [B,n_out,HW] = sigmoid(x.w + b) (n_out = 2, C % 8 == 0). */
+int sb_det_classifier(int dtype, const void* x, const void* w, const void* b, void* out, long long P, int C, int HW, int n_out,
+                      void* stream);
 int sb_lite_mla(int dtype, const void* qkv_a, const void* qkv_b, void* out, int B, int HW, int heads, int dim, float eps,
                 void* stream);
 

@@ -230,6 +230,54 @@ int sb_dwconv_nhwc(int dtype, const void* in, const void* w, const float* bias, 
   return det_dwconv(dtype, in, w, bias, out, B, H, W, C, ks, stride, pad, act, static_cast<cudaStream_t>(stream));
 }
 
+int sb_det_stem_conv(int dtype, const void* in, int in_f32, const float* w, const float* bias, void* out, int B, int H, int W,
+                     int cout, void* stream) {
+  if (!in || !w || !bias || !out) { set_error("sb_det_stem_conv: null argument"); return -1; }
+  return det_stem_conv(dtype, in, in_f32, w, bias, out, B, H, W, cout, static_cast<cudaStream_t>(stream));
+}
+
+int sb_det_fmb_fused(int dtype, const void* in, const void* w1, const float* bias1, const void* w2, const float* bias2,
+                     const void* residual, void* out, int n_img, int H, int W, int Cin, int Cmid, int Cout, int stride,
+                     void* stream) {
+  if (!in || !w1 || !bias1 || !w2 || !bias2 || !out) { set_error("sb_det_fmb_fused: null argument"); return -1; }
+  return fmb_fused(dtype, in, w1, bias1, w2, bias2, residual, out, n_img, H, W, Cin, Cmid, Cout, stride,
+                   static_cast<cudaStream_t>(stream));
+}
+
+// the source list of an UPCAT op: 1..4 non-null maps with their sizes and channel offsets
+static bool upcat_sources_ok(const void* const* srcs, const int* hs, const int* ws, const int* ch_off, int n_src) {
+  if (!srcs || !hs || !ws || !ch_off || n_src < 1 || n_src > 4) return false;
+  for (int i = 0; i < n_src; ++i)
+    if (!srcs[i]) return false;
+  return true;
+}
+
+int sb_det_head_fused(int dtype, const void* const* srcs, const int* hs, const int* ws, const int* ch_off, int n_src, int CS,
+                      const void* fuse_w, const float* fuse_bias, const void* cls_w, const void* cls_b, void* logits, int B,
+                      int HO, int WO, void* stream) {
+  if (!upcat_sources_ok(srcs, hs, ws, ch_off, n_src) || !fuse_w || !fuse_bias || !cls_w || !cls_b || !logits) {
+    set_error("sb_det_head_fused: null argument or bad source count");
+    return -1;
+  }
+  return det_head_fused(dtype, srcs, hs, ws, ch_off, n_src, CS, fuse_w, fuse_bias, cls_w, cls_b, logits, B, HO, WO,
+                        static_cast<cudaStream_t>(stream));
+}
+
+int sb_det_upsample_cat(int dtype, const void* const* srcs, const int* hs, const int* ws, const int* ch_off, int n_src, int CS,
+                        void* dst, int B, int HO, int WO, void* stream) {
+  if (!upcat_sources_ok(srcs, hs, ws, ch_off, n_src) || !dst) {
+    set_error("sb_det_upsample_cat: null argument or bad source count");
+    return -1;
+  }
+  return det_upsample_cat(dtype, srcs, hs, ws, ch_off, n_src, CS, dst, B, HO, WO, static_cast<cudaStream_t>(stream));
+}
+
+int sb_det_classifier(int dtype, const void* x, const void* w, const void* b, void* out, long long P, int C, int HW, int n_out,
+                      void* stream) {
+  if (!x || !w || !b || !out) { set_error("sb_det_classifier: null argument"); return -1; }
+  return det_classifier(dtype, x, w, b, out, P, C, HW, n_out, static_cast<cudaStream_t>(stream));
+}
+
 int sb_gemm_grouped(int dtype, const void* A, int lda, int a_cols, const void* W, int ldw, void* C, int ldc, int M, int N,
                     int Kpad, int group_k, int group_n, void* stream) {
   GemmArgs g;

@@ -363,6 +363,15 @@ int det_lite_mla(int dtype, const void* qkv_a, const void* qkv_b, void* out, int
   return launch_ok();
 }
 
+// bilinear blend with a pinned operation order (no compiler-chosen FMA contraction): the decode-head up-sampler, the fp32
+// up-sampler and the post-processing front half must produce the same bits, and so must the fused head's builders
+// (det_head.cu), which evaluate this expression for the integer ratios whose weights are exact in the 16-bit type
+__device__ __forceinline__ float bilerp(float hy, float ly, float hx, float lx, float a, float b, float c, float d) {
+  const float p = __fmaf_rn(lx, b, __fmul_rn(hx, a));
+  const float q = __fmaf_rn(lx, d, __fmul_rn(hx, c));
+  return __fmaf_rn(ly, q, __fmul_rn(hy, p));
+}
+
 // ------------------------------------------------------------------------------------------------ decode-head upsample + concat
 // src maps NHWC [B, hs, ws, CS]; dst NHWC [B, HO, WO, n_src*CS], map i written at channel offset ch_off[i].
 struct UpcatParams {
@@ -426,8 +435,7 @@ __global__ void __launch_bounds__(256) upsample_cat_kernel(const UpcatParams p, 
     T* pe = reinterpret_cast<T*>(&pack);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      float v = hy * (hx * to_f<T>(e00[j]) + lx * to_f<T>(e01[j])) + ly[y] * (hx * to_f<T>(e10[j]) + lx * to_f<T>(e11[j]));
-      pe[j] = from_f<T>(v);
+      pe[j] = from_f<T>(bilerp(hy, ly[y], hx, lx, to_f<T>(e00[j]), to_f<T>(e01[j]), to_f<T>(e10[j]), to_f<T>(e11[j])));
     }
     *reinterpret_cast<uint4*>(drow + static_cast<size_t>(oy0 + y) * p.WO * CT) = pack;
   }
@@ -492,14 +500,6 @@ int det_classifier(int dtype, const void* x, const void* w, const void* b, void*
     classifier_kernel<__nv_bfloat16, 2><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)w,
                                                               (const __nv_bfloat16*)b, (__nv_bfloat16*)out, P, C, HW);
   return launch_ok();
-}
-
-// bilinear blend with a pinned operation order (no compiler-chosen FMA contraction): the fp32 up-sampler and the
-// post-processing front half must produce the same bits
-__device__ __forceinline__ float bilerp(float hy, float ly, float hx, float lx, float a, float b, float c, float d) {
-  const float p = __fmaf_rn(lx, b, __fmul_rn(hx, a));
-  const float q = __fmaf_rn(lx, d, __fmul_rn(hx, c));
-  return __fmaf_rn(ly, q, __fmul_rn(hy, p));
 }
 
 // ------------------------------------------------------------------------------------------------ x4 bilinear to fp32 (NCHW)

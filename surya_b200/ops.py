@@ -203,13 +203,22 @@ def small_head(x, w, b, sigmoid=True, box_scale=None):
 
 
 # ------------------------------------------------------------------------------------------------ detection ops (NHWC)
-def conv2d_nhwc(x, w, bias=None, residual=None, ksize=3, stride=1, pad=1, act="none"):
+def _out(out, shape, like, dtype=None):
+    """`out` (dense, checked) or a new tensor: the detection kernels write their outputs densely at the given pointer."""
+    dtype = like.dtype if dtype is None else dtype
+    if out is None:
+        return torch.empty(shape, device=like.device, dtype=dtype)
+    assert tuple(out.shape) == tuple(shape) and out.dtype == dtype and out.is_contiguous(), "out: wrong shape, dtype or layout"
+    return out
+
+
+def conv2d_nhwc(x, w, bias=None, residual=None, ksize=3, stride=1, pad=1, act="none", out=None):
     """x [N,H,W,Cin], w [Cout, k*k*Cin] (K ordered r,s,c), bias fp32 [Cout] -> [N,Ho,Wo,Cout]."""
     lib = _lib.load()
     N, H, W, Cin = x.shape
     Cout = w.shape[0]
     Ho, Wo = (H + 2 * pad - ksize) // stride + 1, (W + 2 * pad - ksize) // stride + 1
-    out = torch.empty((N, Ho, Wo, Cout), device=x.device, dtype=x.dtype)
+    out = _out(out, (N, Ho, Wo, Cout), x)
     check(lib.sb_conv2d_nhwc(dt_code(x.dtype), ptr(x), ptr(w), ptr(bias), ptr(residual), ptr(out), c_int(N), c_int(H), c_int(W),
                              c_int(Cin), c_int(Cout), c_int(ksize), c_int(stride), c_int(pad), c_int(ACT[act]), stream_ptr()),
           "sb_conv2d_nhwc")
@@ -224,6 +233,81 @@ def dwconv_nhwc(x, w, bias=None, ksize=3, stride=1, pad=1, act="none"):
     out = torch.empty((N, Ho, Wo, C), device=x.device, dtype=x.dtype)
     check(lib.sb_dwconv_nhwc(dt_code(x.dtype), ptr(x), ptr(w), ptr(bias), ptr(out), c_int(N), c_int(H), c_int(W), c_int(C),
                              c_int(ksize), c_int(stride), c_int(pad), c_int(ACT[act]), stream_ptr()), "sb_dwconv_nhwc")
+    return out
+
+
+def det_stem_conv(x, w, bias, dtype=None, out=None):
+    """Stem: x NCHW [B,3,H,W] (fp32, converted to `dtype` in the kernel, or 16-bit), w fp32 [Cout, 27] (K ordered r,s,c),
+    bias fp32 [Cout] -> 3x3 stride-2 conv + Hardswish, NHWC [B,H/2,W/2,Cout]."""
+    lib = _lib.load()
+    B, _, H, W = x.shape
+    dtype = x.dtype if dtype is None else dtype
+    Cout = w.shape[0]
+    assert w.dtype == torch.float32 and bias.dtype == torch.float32
+    out = _out(out, (B, H // 2, W // 2, Cout), x, dtype)
+    check(lib.sb_det_stem_conv(dt_code(dtype), ptr(x), c_int(1 if x.dtype == torch.float32 else 0), ptr(w), ptr(bias), ptr(out),
+                               c_int(B), c_int(H), c_int(W), c_int(Cout), stream_ptr()), "sb_det_stem_conv")
+    return out
+
+
+def det_fmb_fused(x, w1, b1, w2, b2, residual=None, stride=1, out=None):
+    """FusedMBConv: x [N,H,W,Cin], w1 [Cmid, 9*Cin] (K ordered r,s,c), b1 fp32 [Cmid], w2 [Cout, Cmid], b2 fp32 [Cout]
+    -> 3x3 conv + b1, Hardswish, 1x1 conv + b2 (+ residual) -> [N,Ho,Wo,Cout] (pad 1)."""
+    lib = _lib.load()
+    N, H, W, Cin = x.shape
+    Cmid, Cout = w1.shape[0], w2.shape[0]
+    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+    out = _out(out, (N, Ho, Wo, Cout), x)
+    check(lib.sb_det_fmb_fused(dt_code(x.dtype), ptr(x), ptr(w1), ptr(b1), ptr(w2), ptr(b2), ptr(residual), ptr(out), c_int(N),
+                               c_int(H), c_int(W), c_int(Cin), c_int(Cmid), c_int(Cout), c_int(stride), stream_ptr()),
+          "sb_det_fmb_fused")
+    return out
+
+
+def _sources(srcs, ch_off):
+    n = len(srcs)
+    arr = (c_void_p * n)(*[s.data_ptr() for s in srcs])
+    hs = (c_int * n)(*[s.shape[1] for s in srcs])
+    ws = (c_int * n)(*[s.shape[2] for s in srcs])
+    off = (c_int * n)(*ch_off)
+    for s in srcs:
+        assert s.is_contiguous() and s.shape[3] == srcs[0].shape[3]
+    return arr, hs, ws, off
+
+
+def det_head_fused(srcs, ch_off, fuse_w, fuse_b, cls_w, cls_b, HO, WO, out=None):
+    """Decode head: srcs NHWC [B,hs,ws,CS] at channel ch_off[i] of the concat, bilinear to HO x WO -> fuse_w [512,512] + fuse_b
+    fp32, ReLU -> cls_w [2,512] + cls_b [2] -> sigmoid -> NCHW [B,2,HO,WO]."""
+    lib = _lib.load()
+    B, CS = srcs[0].shape[0], srcs[0].shape[3]
+    out = _out(out, (B, cls_w.shape[0], HO, WO), srcs[0])
+    arr, hs, ws, off = _sources(srcs, ch_off)
+    check(lib.sb_det_head_fused(dt_code(srcs[0].dtype), arr, hs, ws, off, c_int(len(srcs)), c_int(CS), ptr(fuse_w), ptr(fuse_b),
+                                ptr(cls_w), ptr(cls_b), ptr(out), c_int(B), c_int(HO), c_int(WO), stream_ptr()),
+          "sb_det_head_fused")
+    return out
+
+
+def det_upsample_cat(srcs, ch_off, HO, WO, out=None):
+    """srcs NHWC [B,hs,ws,CS] -> bilinear (align_corners=False) to HO x WO, concatenated at channel ch_off[i]:
+    [B,HO,WO,len(srcs)*CS]."""
+    lib = _lib.load()
+    B, CS = srcs[0].shape[0], srcs[0].shape[3]
+    out = _out(out, (B, HO, WO, len(srcs) * CS), srcs[0])
+    arr, hs, ws, off = _sources(srcs, ch_off)
+    check(lib.sb_det_upsample_cat(dt_code(srcs[0].dtype), arr, hs, ws, off, c_int(len(srcs)), c_int(CS), ptr(out), c_int(B),
+                                  c_int(HO), c_int(WO), stream_ptr()), "sb_det_upsample_cat")
+    return out
+
+
+def det_classifier(x, w, b, HW, out=None):
+    """x [P, C] (P = B*HW pixels, NHWC order), w [n_out, C], b [n_out] -> sigmoid(x w^T + b) as NCHW [B, n_out, HW]."""
+    lib = _lib.load()
+    P, C = x.shape
+    n_out = w.shape[0]
+    out = _out(out, (P // HW, n_out, HW), x)
+    check(lib.sb_det_classifier(dt_code(x.dtype), ptr(x), ptr(w), ptr(b), ptr(out), ctypes.c_longlong(P), c_int(C), c_int(HW),
+                                c_int(n_out), stream_ptr()), "sb_det_classifier")
     return out
 
 

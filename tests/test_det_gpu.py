@@ -373,7 +373,10 @@ def test_fused_kernels_equal_unfused_ops(built_lib, switch, size, tmp_path):
                          classifier: same rounding points, only the fp32 summation order of the 512-long classifier dot differs;
       SB_FMB_FUSED       conv_fmb.cu (3x3 expand + Hardswish + 1x1 project + shortcut, back-to-back GEMM) vs conv_igemm -> gemm:
                          same rounding points and the same k order.
-    Heatmaps must agree to one fp16 ulp.  320x448 gives partial tiles in both directions at every stage."""
+    The fused MBConv must give the same bits.  For the head, a logit that flips by one ulp moves the sigmoid output by at most
+    a quarter of the logit's ulp and the output rounds once more: never more than one ulp of the [0.5, 1) binade (2^-11), and
+    the flips are rare (99.97 % of values were bit-equal on an H100).  320x448 gives partial tiles in both directions at every
+    stage."""
     import os
     import subprocess
     import sys
@@ -392,4 +395,6 @@ def test_fused_kernels_equal_unfused_ops(built_lib, switch, size, tmp_path):
     diff = (fused - unfused).abs()
     frac_equal = (diff == 0).float().mean().item()
     print(f"{switch}={on} vs 0 at {size}: max |diff| {diff.max().item():.3g}, identical {100 * frac_equal:.2f} %")
-    assert diff.max().item() <= 2 ** -10 and frac_equal > 0.98
+    if switch == "SB_FMB_FUSED":
+        assert torch.equal(fused, unfused)
+    assert diff.max().item() <= 2 ** -11 and frac_equal >= 0.999
