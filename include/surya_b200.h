@@ -80,17 +80,23 @@ int sb_rope_vision(int dtype, void* qkv, int ld, const int* pos_rc, const float*
                    void* stream);
 
 /* apply_rotary_pos_emb (decoder/__init__.py:60-84, 346-361) + DynamicCache.update without the torch.cat
- * (decoder/__init__.py:190-195): rotates q,k in place and writes k,v into cache[slot][kv_head][pos][:]. */
+ * (decoder/__init__.py:190-195): rotates q,k in place and writes k,v into cache[slot][kv_head][pos][:].  A token with pos
+ * outside [0, s_max) is rotated but writes nothing to the cache. */
 int sb_rope_kv_append(int dtype, void* qkv, int ld, const int* tok_pos, const int* tok_slot, const float* inv_freq,
                       void* kcache, void* vcache, int n_tok, int nh, int nkv, int d, int s_max, void* stream);
 
 /* flash_attn_varlen_func / SDPA over packed sequences (encoder/__init__.py:174-176, 400-406;
- * flash_attn_utils.py:106-154).  Head h of q at column q_col0 + h*d of a row-major matrix with pitch ldq. */
+ * flash_attn_utils.py:106-154).  Head h of q at column q_col0 + h*d of a row-major matrix with pitch ldq.
+ * n_heads must be a positive multiple of n_kv_heads.  q, k and v are read as 16-byte vectors: their bases must be 16-byte
+ * aligned and ldq / ldk / ldv multiples of 8 elements; out is stored in 4-byte pairs: 4-byte aligned base, even ldo.
+ * No sequence may be longer than max_len: rows past ceil(max_len / 64) * 64 are never written. */
 int sb_attn_varlen(int dtype, const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out,
                    int ldo, const int* seq_start, const int* seq_len, int n_seq, int max_len, int n_heads,
                    int n_kv_heads, int head_dim, int causal, float scale, void* stream);
 
-/* flash_attn_with_kvcache / SDPA decode step (flash_attn_utils.py:157-188) fused with RoPE and cache append. */
+/* flash_attn_with_kvcache / SDPA decode step (flash_attn_utils.py:157-188) fused with RoPE and cache append.
+ * n_heads must be a positive multiple of n_kv_heads.  A row with pos outside [0, s_max) outputs zeros and leaves the cache
+ * unchanged.  An s_max whose scores do not fit in shared memory is an error (-3). */
 int sb_decode_attn(int dtype, const void* qkv, int ld, void* kcache, void* vcache, const int* slot, const int* pos,
                    const float* inv_freq, void* out, int ldo, int batch, int n_heads, int n_kv_heads, int head_dim,
                    int s_max, float scale, void* stream);
@@ -343,7 +349,8 @@ int sb_swin_window_attn(int dtype, const void* qkv, const float* qkv_bias, const
 /* BboxEmbedding (layout/model/decoder.py:36-57): tables = 15 device pointers (w,h,cx,cy,xskew,yskew,x1,y1,...,y4,label). */
 int sb_bbox_embed_sum(int dtype, const long long* boxes, const void* const* tables, void* out, int n, int Hd, int bbox_size,
                       void* stream);
-/* q_len = 1 attention over a fixed K/V set with explicit strides (ADETR cross-attention, adetr/decoder.py:150-194). */
+/* q_len = 1 attention over a fixed K/V set with explicit strides (ADETR cross-attention, adetr/decoder.py:150-194).
+ * nh must be a positive multiple of nkv (group 1, 2 or 4) and n_keys positive. */
 int sb_attn_single_query(int dtype, const void* q, int ldq, const void* K, const void* V, long long batch_stride,
                          long long head_stride, long long token_stride, void* out, int ldo, int B, int nh, int nkv, int head_dim,
                          int n_keys, float scale, void* stream);

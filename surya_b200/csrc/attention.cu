@@ -251,8 +251,15 @@ static int dispatch_varlen(const AttnArgs& a, cudaStream_t st) {
 
 int attn_varlen(const AttnArgs& a, cudaStream_t st) {
   if (a.n_seq <= 0 || a.max_len <= 0) return 0;
-  if (a.n_heads % a.n_kv_heads) { set_error("attn_varlen: n_heads must be a multiple of n_kv_heads"); return -1; }
+  if (a.n_kv_heads <= 0 || a.n_heads % a.n_kv_heads) {
+    set_error("attn_varlen: n_heads must be a positive multiple of n_kv_heads"); return -1;
+  }
   if (a.ldq % 8 || a.ldk % 8 || a.ldv % 8 || a.ldo % 2) { set_error("attn_varlen: pitches must be 16B multiples"); return -1; }
+  // q / k / v rows are read as 16-byte vectors and out is stored as 4-byte pairs (the pitches are checked above)
+  if ((reinterpret_cast<uintptr_t>(a.q) | reinterpret_cast<uintptr_t>(a.k) | reinterpret_cast<uintptr_t>(a.v)) % 16 ||
+      reinterpret_cast<uintptr_t>(a.out) % 4) {
+    set_error("attn_varlen: q, k and v must be 16B aligned and out 4B aligned"); return -1;
+  }
   return a.dtype == DT_BF16 ? dispatch_varlen<__nv_bfloat16>(a, st) : dispatch_varlen<__half>(a, st);
 }
 
@@ -434,6 +441,7 @@ static int launch_decode(const DecodeAttnArgs& a, cudaStream_t st) {
   static size_t attr = 0;
   if (smem > 48 * 1024 && smem > attr) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+      cudaGetLastError();  // clear it: the next launch_ok() would report this error as its own
       set_error("decode_attn: %zu bytes of shared memory exceed the device limit (s_max too large)", smem);
       return -3;
     }
@@ -472,7 +480,9 @@ static int dispatch_decode(const DecodeAttnArgs& a, cudaStream_t st) {
 
 int decode_attn(const DecodeAttnArgs& a, cudaStream_t st) {
   if (a.batch <= 0) return 0;
-  if (a.n_heads % a.n_kv_heads) { set_error("decode_attn: n_heads must be a multiple of n_kv_heads"); return -1; }
+  if (a.n_kv_heads <= 0 || a.n_heads % a.n_kv_heads) {
+    set_error("decode_attn: n_heads must be a positive multiple of n_kv_heads"); return -1;
+  }
   return a.dtype == DT_BF16 ? dispatch_decode<__nv_bfloat16>(a, st) : dispatch_decode<__half>(a, st);
 }
 

@@ -634,6 +634,8 @@ static int launch_sq(const void* q, int ldq, const void* K, const void* V, long 
 int attn_single_query(int dtype, const void* q, int ldq, const void* K, const void* V, long long bs, long long hs, long long ts,
                       void* out, int ldo, int B, int nh, int nkv, int head_dim, int n_keys, float scale, cudaStream_t st) {
   if (head_dim != 64) { set_error("attn_single_query: head_dim 64 is instantiated (got %d)", head_dim); return -1; }
+  if (nkv <= 0 || nh % nkv) { set_error("attn_single_query: nh (%d) must be a positive multiple of nkv (%d)", nh, nkv); return -1; }
+  if (n_keys <= 0) { set_error("attn_single_query: n_keys must be positive (got %d)", n_keys); return -1; }
   const int G = nh / nkv;
 #define SQ(T_) \
   (G == 1 ? launch_sq<T_, 1>(q, ldq, K, V, bs, hs, ts, out, ldo, B, nkv, n_keys, scale, st) : \

@@ -450,7 +450,9 @@ int rope_vision(int dtype, void* qkv, int ld, const int* pos_rc, const float* in
 // ------------------------------------------------------------------------------------------ decoder RoPE + KV append
 // qkv row = [q(nh*d) | k(nkv*d) | v(nkv*d)].  cos/sin are computed in fp32, cast to T, and the rotation is
 // evaluated in T arithmetic with three roundings (mul, mul, add) like the eager reference.  q and k are rotated
-// in place; rotated k and v are also written to the slot cache at index `pos`.
+// in place; rotated k and v are also written to the slot cache at index `pos`.  A token whose pos is outside
+// [0, s_max) is still rotated but writes nothing to the cache (host-side callers reject it before launching): its
+// row would land in the next kv head's or slot's rows, the same bound decode_attn_kernel enforces.
 template <typename T>
 __device__ __forceinline__ void rope_pair_T(float x1, float x2, float c, float s, float& o1, float& o2) {
   // o1 = x1*c + (-x2)*s ; o2 = x2*c + x1*s   (each product and the sum rounded to T)
@@ -468,6 +470,7 @@ __global__ void rope_kv_append_kernel(T* __restrict__ qkv, int ld, const int* __
   const int half = d >> 1;
   const int pos = tok_pos[tok];
   const int slot = tok_slot[tok];
+  const bool in_cache = pos >= 0 && pos < s_max;
   T* row = qkv + static_cast<size_t>(tok) * ld;
   __shared__ float s_cos[128], s_sin[128];
   for (int i = threadIdx.x; i < half; i += blockDim.x) {
@@ -487,13 +490,14 @@ __global__ void rope_kv_append_kernel(T* __restrict__ qkv, int ld, const int* __
     rope_pair_T<T>(x1, x2, c, s, o1, o2);
     h[i] = from_f<T>(o1);
     h[i + half] = from_f<T>(o2);
-    if (hh >= nh) {
+    if (hh >= nh && in_cache) {
       int kvh = hh - nh;
       T* kc = kcache + ((static_cast<size_t>(slot) * nkv + kvh) * s_max + pos) * d;
       kc[i] = from_f<T>(o1);
       kc[i + half] = from_f<T>(o2);
     }
   }
+  if (!in_cache) return;
   const T* vrow = row + (nh + nkv) * d;
   for (int idx = threadIdx.x; idx < nkv * d; idx += blockDim.x) {
     int kvh = idx / d, i = idx % d;

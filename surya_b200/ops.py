@@ -407,11 +407,13 @@ def bbox_embed_sum(boxes, tables, hidden, bbox_size, dtype):
     return out
 
 
-def attn_single_query(q, kv, n_keys, nh, nkv, hd, scale):
-    """q [B, nh*hd]; kv [B*n_keys, 2*nkv*hd] = per token (K heads | V heads), i.e. the fused cross K/V projection output."""
+def attn_single_query(q, kv, n_keys, nh, nkv, hd, scale, out=None):
+    """q [B, nh*hd]; kv [B*n_keys, 2*nkv*hd] = per token (K heads | V heads), i.e. the fused cross K/V projection output.
+    out: optional row-major [B, nh*hd] view (e.g. a column window of a wider buffer)."""
     lib = _lib.load()
     B = q.shape[0]
-    out = torch.empty_like(q)
+    if out is None:
+        out = torch.empty((B, nh * hd), device=q.device, dtype=q.dtype)
     row = 2 * nkv * hd
     esz = kv.element_size()
     kptr = kv.data_ptr()

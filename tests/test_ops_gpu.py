@@ -303,6 +303,26 @@ def _attn_ref(q, k, v, lens, causal, scale, group):
     return torch.cat(outs, 0)
 
 
+def _attn_bound(got, q, k, v, scale, vis, dtype, what):
+    """Attention output `got` [n, d] of q [n, d] over k, v [m, d] (the exact 16-bit values the kernel read, visibility vis
+    [n, m]) against float64 softmax(scale q k^T) v, with the worst-case bound of tests/test_attention_gpu.py (`_eps` there
+    derives eps): |got - O*| <= u|O*| + (u + eps) A + eps |O*| + tiny, A = sum_j p*_j |v_j|."""
+    q, k, v = q.double(), k.double(), v.double()
+    u = _ulp(dtype)
+    s = ((q @ k.T) * scale).masked_fill(~vis, -math.inf)
+    m = s.amax(-1, keepdim=True)
+    w = torch.exp(s - m)
+    l = w.sum(-1, keepdim=True)
+    O, A = (w / l) @ v, (w / l) @ v.abs()
+    R = (m - s).masked_fill(~vis, 0.0).amax(-1, keepdim=True).clamp(max=64.0)
+    dot = ((q.abs() @ k.abs().T) * scale).masked_fill(~vis, 0.0).amax(-1, keepdim=True)
+    eps = 2.0 * (2.0 * 2.0 ** -23 * (q.shape[1] + 2) * dot + 2.0 ** -21 + 2.0 ** -23 * R) + vis.sum(-1, keepdim=True) * 2.0 ** -23
+    tiny = (2.0 ** -134 if dtype == torch.bfloat16 else 2.0 ** -25) * (vis.double() @ v.abs()) / l
+    bound = (u * O.abs() + (u + eps) * A + eps * O.abs() + tiny) * (1.0 + 4.0 * u)
+    err = (got.double() - O).abs()
+    assert bool((err <= bound).all()), f"{what}: max err {err.max().item():.3g} beyond the float64 bound"
+
+
 @pytest.mark.parametrize("dtype", DT)
 @pytest.mark.parametrize("d,nh,nkv,causal,lens", [
     (80, 4, 4, False, [32, 32, 64, 17, 160, 1]),
@@ -328,6 +348,15 @@ def test_attn_varlen(built_lib, dtype, d, nh, nkv, causal, lens):
                     causal, scale, nh // nkv).reshape(T, nh * d)
     err = (out.float() - ref).abs().max().item()
     assert err < (0.03 if dtype == torch.bfloat16 else 0.005), f"attn_varlen max err {err}"
+    G = nh // nkv
+    for st, L in zip(starts.tolist(), lens):
+        vis = torch.ones(L, L, dtype=torch.bool, device="cuda")
+        if causal:
+            vis = vis.tril()
+        for h in range(nh):
+            kv = slice((h // G) * d, (h // G + 1) * d)
+            _attn_bound(out[st:st + L, h * d:(h + 1) * d], q[st:st + L, h * d:(h + 1) * d], k[st:st + L, kv],
+                        v[st:st + L, kv], scale, vis, dtype, f"attn_varlen seq@{st} head {h}")
 
 
 @pytest.mark.parametrize("dtype", DT)
@@ -373,6 +402,9 @@ def test_decode_attn_and_rope_append(built_lib, dtype, d, nh, nkv):
     slot = torch.tensor(slot_ids, device="cuda", dtype=torch.int32)
     pos = torch.tensor(lens, device="cuda", dtype=torch.int32)
     qkv1 = torch.randn(B, width, device="cuda", generator=g).to(dtype)
+    # the rotated q the kernel used: rope_kv_append rotates the same rows with the same rounding points (own cache copies)
+    qrot = qkv1.clone()
+    ops.rope_kv_append_(qrot, pos, slot, inv_freq, kc.clone(), vc.clone(), nh, nkv, d)
     out = ops.decode_attn(qkv1, kc, vc, slot, pos, inv_freq, nh, nkv, d, d ** -0.5)
     torch.cuda.synchronize()
     qk1 = rope_T(qkv1[:, : (nh + nkv) * d].reshape(B, nh + nkv, d), pos)
@@ -388,6 +420,11 @@ def test_decode_attn_and_rope_append(built_lib, dtype, d, nh, nkv):
         ref = torch.einsum("hk,hkd->hd", sc.softmax(-1), V).reshape(-1)
         err = (out[b].float() - ref).abs().max().item()
         assert err < (0.03 if dtype == torch.bfloat16 else 0.005), f"decode_attn row {b} err {err}"
+        vis = torch.ones(group, L + 1, dtype=torch.bool, device="cuda")
+        for kvh in range(nkv):
+            _attn_bound(out[b, kvh * group * d:(kvh + 1) * group * d].reshape(group, d),
+                        qrot[b, kvh * group * d:(kvh + 1) * group * d].reshape(group, d), kc[s, kvh, :L + 1], vc[s, kvh, :L + 1],
+                        d ** -0.5, vis, dtype, f"decode_attn row {b} kv head {kvh}")
 
 
 @pytest.mark.parametrize("dtype", DT)
