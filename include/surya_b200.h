@@ -46,10 +46,14 @@ long long sb_launch_count(void);
  * Rejected with a negative code (see sb_last_error): A, W, C or residual not 16-byte aligned, an lda / ldw pitch that is not
  * a multiple of 16 bytes, swiglu with a residual, out_f32 with a residual or with swiglu.  C may be the residual (in place).
  * Preceding kernels on the stream may still be running when this one starts (programmatic dependent launch); A, W, bias and
- * residual are read only after they have completed. */
+ * residual are read only after they have completed.
+ * decode: 0 = the kernels above; 1 = the decode-step kernel (M <= 256, the 16-bit staged epilogue only; bit-identical to the
+ * plain kernel at any tile width), tile width from its per-shape table unless force_bn is 32, 64 or 128.  M <= 16 still takes
+ * the skinny kernel when it applies.  Refused with decode = 1: M > 256, out_f32, forced split-K (force_bn >= 1000), other tile
+ * widths, N % 8 != 0 (N % 16 with swiglu), ldc or ldr not a multiple of 8; any decode value other than 0 and 1. */
 int sb_gemm(int dtype, const void* A, int lda, const void* W, int ldw, void* C, int ldc, int M, int N, int K,
             const float* bias, const void* residual, int ldr, int act, int swiglu, int out_f32, int force_bn,
-            void* stream);
+            int decode, void* stream);
 
 /* nn.Linear applied to Qwen2RMSNorm(x) with the norm folded into the GEMM (decoder/__init__.py:241-258 followed by
  * :147-158 / :37-50, and the final norm + lm_head / bbox_head of surya/common/surya/__init__.py:323-330):
@@ -58,10 +62,11 @@ int sb_gemm(int dtype, const void* A, int lda, const void* W, int ldw, void* C, 
  *   inside the kernel from the A tiles with rms_eps (no separate pass over A; used by the decode steps).
  * Optional online argmax epilogue (am_val != NULL): per (row, n-tile) partials (max logit, first argmax, sum exp(l - max)) of
  * the 16-bit-rounded outputs into [M, am_ld] arrays, tile width = sb_gemm_argmax_tile(M, N); C is written only if store_c —
- * RecognitionPredictor.process_outputs (surya/recognition/__init__.py:294-324) needs argmax and max-softmax only. */
+ * RecognitionPredictor.process_outputs (surya/recognition/__init__.py:294-324) needs argmax and max-softmax only.
+ * decode: as for sb_gemm; with the argmax epilogue the tile width stays sb_gemm_argmax_tile(M, N). */
 int sb_gemm_rmsnorm(int dtype, const void* A, int lda, const void* W, int ldw, void* C, int ldc, int M, int N, int K,
                     const float* bias, const void* residual, int ldr, int act, int swiglu, const float* rowscale, float rms_eps,
-                    float* am_val, int* am_idx, float* am_sum, int am_ld, int store_c, int force_bn, void* stream);
+                    float* am_val, int* am_idx, float* am_sum, int am_ld, int store_c, int force_bn, int decode, void* stream);
 int sb_gemm_argmax_tile(int M, int N);
 /* rs[row] = rsqrt(mean(x[row]^2) + eps) in the summation order sb_gemm_rmsnorm's in-kernel pass uses (bit-identical). */
 int sb_row_rstd(int dtype, const void* x, int ldx, float* rs, int rows, int H, float eps, const int* src_rows, void* stream);

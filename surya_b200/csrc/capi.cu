@@ -12,19 +12,21 @@ long long sb_launch_count(void) { return launch_count(); }
 
 int sb_gemm(int dtype, const void* A, int lda, const void* W, int ldw, void* C, int ldc, int M, int N, int K,
             const float* bias, const void* residual, int ldr, int act, int swiglu, int out_f32, int force_bn,
-            void* stream) {
+            int decode, void* stream) {
   GemmArgs a;
   a.dtype = dtype; a.A = A; a.lda = lda; a.W = W; a.ldw = ldw; a.C = C; a.ldc = ldc;
   a.M = M; a.N = N; a.K = K; a.bias = bias; a.residual = residual; a.ldr = ldr;
   a.act = act; a.swiglu = swiglu; a.out_f32 = out_f32;
   a.force_bn = force_bn < 0 ? 0 : force_bn;
   a.allow_splitk = force_bn < 0 ? 1 : 0;
+  a.decode = decode;
   return gemm_launch(a, static_cast<cudaStream_t>(stream));
 }
 
 int sb_gemm_rmsnorm(int dtype, const void* A, int lda, const void* W, int ldw, void* C, int ldc, int M, int N, int K,
                     const float* bias, const void* residual, int ldr, int act, int swiglu, const float* rowscale, float rms_eps,
-                    float* am_val, int* am_idx, float* am_sum, int am_ld, int store_c, int force_bn, void* stream) {
+                    float* am_val, int* am_idx, float* am_sum, int am_ld, int store_c, int force_bn, int decode,
+                    void* stream) {
   GemmArgs a;
   a.dtype = dtype; a.A = A; a.lda = lda; a.W = W; a.ldw = ldw; a.C = C; a.ldc = ldc;
   a.M = M; a.N = N; a.K = K; a.bias = bias; a.residual = residual; a.ldr = ldr;
@@ -34,6 +36,7 @@ int sb_gemm_rmsnorm(int dtype, const void* A, int lda, const void* W, int ldw, v
   if (!rowscale) { a.ssq_inline = 1; a.ssq_eps = rms_eps; a.ssq_k = K; }
   a.am_val = am_val; a.am_idx = am_idx; a.am_sum = am_sum; a.am_ld = am_ld;
   a.store_c = am_val ? store_c : 1;
+  a.decode = decode;
   return gemm_launch(a, static_cast<cudaStream_t>(stream));
 }
 

@@ -45,12 +45,19 @@ struct GemmArgs {
   float* am_sum = nullptr;
   int am_ld = 0;
   int store_c = 1;
+  // decode-step kernel (gemm_decode.cu, M <= 256): 0 = off, 1 = on (tile width from its per-shape table unless force_bn).
+  // Same bits as the plain kernel.
+  int decode = 0;
 };
 // M <= 16 rows: mma.sync kernel without the wgmma pipeline set-up costs (gemm_skinny.cu); gemm_launch routes to it when it applies.
 bool gemm_skinny_ok(const GemmArgs& a);
 int gemm_skinny_launch(const GemmArgs& a, cudaStream_t stream);
 // Tile width gemm_launch will use for an argmax-epilogue launch of this shape (partials per row = ceil(N / width)).
 int gemm_argmax_tile(int M, int N);
+
+// Decode-step kernel: argument check (the combinations it cannot take are refused) and launch.
+int gemm_decode_check(const GemmArgs& a);
+int gemm_decode_launch(const GemmArgs& a, cudaStream_t stream);
 
 // Returns cudaSuccess or an error; sets a message retrievable through sb_last_error().
 int gemm_launch(const GemmArgs& a, cudaStream_t stream);

@@ -458,7 +458,12 @@ int gemm_launch(const GemmArgs& a, cudaStream_t stream) {
     return -13;
   }
   if (a.dtype != DT_BF16 && a.dtype != DT_F16) { set_error("unsupported dtype %d", a.dtype); return -14; }
+  if (a.decode) {
+    const int rc = gemm_decode_check(a);
+    if (rc) return rc;
+  }
   if (gemm_skinny_ok(a)) return gemm_skinny_launch(a, stream);
+  if (a.decode) return gemm_decode_launch(a, stream);
   if (a.dtype == DT_BF16) return launch_typed<__nv_bfloat16>(a, stream);
   return launch_typed<__half>(a, stream);
 }

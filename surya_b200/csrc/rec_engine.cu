@@ -71,7 +71,7 @@ static size_t al256(size_t v) { return (v + 255) & ~size_t(255); }
 // inside the GEMM from the A tiles (decode steps, lm_head)
 static int linear(const sb_rec_engine* e, const void* A, int lda, const void* Wt, int ldw, void* C, int ldc, int M, int N,
                   int K, const void* bias_f32, const void* residual, int ldr, int act, int swiglu, cudaStream_t st,
-                  int allow_splitk = 0, int norm = 0) {
+                  int allow_splitk = 0, int norm = 0, int decode = 0) {
   GemmArgs a;
   if (norm == 1) a.rowscale = e->rs;
   if (norm == 2) { a.ssq_inline = 1; a.ssq_eps = e->c.rms_eps; a.ssq_k = K; }
@@ -82,6 +82,7 @@ static int linear(const sb_rec_engine* e, const void* A, int lda, const void* Wt
   a.residual = residual; a.ldr = ldr; a.act = act; a.swiglu = swiglu;
   a.w_constant = 1;   // engine weights are never written after packing
   a.allow_splitk = allow_splitk;
+  a.decode = decode;
   return gemm_launch(a, st);
 }
 
@@ -164,6 +165,7 @@ static int run_heads(sb_rec_engine* e, void* hidden, int rows, const HeadOut& o,
   a.rowscale = e->rs;
   a.am_val = e->am_val; a.am_idx = e->am_idx; a.am_sum = e->am_sum; a.am_ld = e->am_ld;
   a.store_c = o.logits ? 1 : 0;
+  a.decode = rows <= 256 ? 1 : 0;   // decode-step kernel (gemm_decode.cu): same bits, faster at these shapes
   CK(gemm_launch(a, st));
   DecodeTailArgs t;
   t.rows = rows;
@@ -237,19 +239,21 @@ static int run_decode_step(sb_rec_engine* e, const long long* ids, const int* sl
   const int Q = (nh + 2 * nkv) * hd;
   const int dt = c.dtype;
   void* x = e->x;
+  // qkv, o and gate/up take the decode-step kernel (gemm_decode.cu, same bits); the down projection keeps split-K
+  const int dec = B <= 256 ? 1 : 0;
   if (ids) CK(embed_rows(dt, ids, e->W(SB_RW_EMBED), x, D, B, D, st));
   for (int l = 0; l < c.dec_layers; ++l) {
     CK(linear(e, x, D, e->WD(l, SB_RWD_QKV_W), D, e->qkv, Q, B, Q, D, e->WD(l, SB_RWD_QKV_B), nullptr, 0, ACT_NONE, 0, st, 0,
-              /*norm=*/2));
+              /*norm=*/2, dec));
     DecodeAttnArgs a;
     a.dtype = dt; a.qkv = e->qkv; a.ld = Q; a.kcache = e->kc(l); a.vcache = e->vc(l); a.slot = slot; a.pos = pos;
     a.inv_freq = static_cast<const float*>(e->W(SB_RW_DEC_INV_FREQ));
     a.out = e->ao; a.ldo = nh * hd; a.batch = B; a.n_heads = nh; a.n_kv_heads = nkv; a.head_dim = hd; a.s_max = c.s_max;
     a.scale = 1.0f / sqrtf(static_cast<float>(hd));
     CK(decode_attn(a, st));
-    CK(linear(e, e->ao, nh * hd, e->WD(l, SB_RWD_O_W), nh * hd, x, D, B, D, nh * hd, nullptr, x, D, ACT_NONE, 0, st));
+    CK(linear(e, e->ao, nh * hd, e->WD(l, SB_RWD_O_W), nh * hd, x, D, B, D, nh * hd, nullptr, x, D, ACT_NONE, 0, st, 0, 0, dec));
     CK(linear(e, x, D, e->WD(l, SB_RWD_GU_W), D, e->act, c.dec_inter_pad, B, 2 * c.dec_inter_pad, D, nullptr, nullptr, 0,
-              ACT_SILU, 1, st, 0, /*norm=*/2));
+              ACT_SILU, 1, st, 0, /*norm=*/2, dec));
     CK(linear(e, e->act, c.dec_inter_pad, e->WD(l, SB_RWD_DOWN_W), c.dec_inter_pad, x, D, B, D, c.dec_inter_pad, nullptr, x, D,
               ACT_NONE, 0, st, /*allow_splitk=*/1));
   }

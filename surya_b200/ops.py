@@ -29,12 +29,13 @@ def _rowmajor(t: torch.Tensor) -> int:
 
 
 def gemm(a, w, bias=None, residual=None, act="none", swiglu=False, out=None, out_f32=False, force_bn=0, splitk=False,
-         rms_eps=None, rowscale=None, argmax=None, argmax_only=False):
+         rms_eps=None, rowscale=None, argmax=None, argmax_only=False, decode=0):
     """out[M, Nout] = epi(a[M,K] @ w[N,K]^T); bias fp32 [N]; see sb_gemm.  splitk=True lets the heuristic use the split-K
     cluster kernel (decode-sized M only).
     rms_eps / rowscale: RMSNorm folded into the GEMM (sb_gemm_rmsnorm): w already carries the norm weight, rows are scaled by
     `rowscale` (fp32 [M]) or by 1/rms computed in the kernel with rms_eps.  argmax: dict filled with the per-tile partials
-    (val, idx, sum) of the online argmax epilogue; argmax_only skips writing the logits."""
+    (val, idx, sum) of the online argmax epilogue; argmax_only skips writing the logits.
+    decode=1: the decode-step kernel for M <= 256 (sb_gemm); same bits as the plain kernel."""
     if splitk and force_bn == 0:
         force_bn = -1
     lib = _lib.load()
@@ -63,12 +64,13 @@ def gemm(a, w, bias=None, residual=None, act="none", swiglu=False, out=None, out
                                   c_int(1 if swiglu else 0), ptr(rowscale), c_float(rms_eps if rms_eps is not None else 0.0),
                                   ptr(am[0]) if am else c_void_p(0), ptr(am[1]) if am else c_void_p(0),
                                   ptr(am[2]) if am else c_void_p(0), c_int(am[0].shape[1] if am else 0),
-                                  c_int(0 if argmax_only else 1), c_int(max(force_bn, 0)), stream_ptr()), "sb_gemm_rmsnorm")
+                                  c_int(0 if argmax_only else 1), c_int(max(force_bn, 0)), c_int(decode), stream_ptr()),
+              "sb_gemm_rmsnorm")
         return out
     check(lib.sb_gemm(dt_code(a.dtype), ptr(a), c_int(_rowmajor(a)), ptr(w), c_int(_rowmajor(w)), ptr(out),
                       c_int(_rowmajor(out)), c_int(M), c_int(N), c_int(K), ptr(bias), ptr(residual),
                       c_int(_rowmajor(residual) if residual is not None else 0), c_int(ACT[act]),
-                      c_int(1 if swiglu else 0), c_int(1 if out_f32 else 0), c_int(force_bn), stream_ptr()), "sb_gemm")
+                      c_int(1 if swiglu else 0), c_int(1 if out_f32 else 0), c_int(force_bn), c_int(decode), stream_ptr()), "sb_gemm")
     return out
 
 
