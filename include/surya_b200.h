@@ -47,9 +47,9 @@ long long sb_launch_count(void);
  * a multiple of 16 bytes, swiglu with a residual, out_f32 with a residual or with swiglu.  C may be the residual (in place).
  * Preceding kernels on the stream may still be running when this one starts (programmatic dependent launch); A, W, bias and
  * residual are read only after they have completed.
- * decode: 0 = the kernels above; 1 = the decode-step kernel (M <= 256, the 16-bit staged epilogue only; bit-identical to the
- * plain kernel at any tile width), tile width from its per-shape table unless force_bn is 32, 64 or 128.  M <= 16 still takes
- * the skinny kernel when it applies.  Refused with decode = 1: M > 256, out_f32, forced split-K (force_bn >= 1000), other tile
+ * decode: 0 = the kernels above; 1 = the GEMM kernel's decode-step variant (M <= 256, the 16-bit staged epilogue only;
+ * bit-identical to the plain variant at any tile width), tile width from its per-shape table unless force_bn is 32, 64 or
+ * 128.  M <= 16 still takes the skinny kernel when it applies.  Refused with decode = 1: M > 256, out_f32, forced split-K (force_bn >= 1000), other tile
  * widths, N % 8 != 0 (N % 16 with swiglu), ldc or ldr not a multiple of 8; any decode value other than 0 and 1. */
 int sb_gemm(int dtype, const void* A, int lda, const void* W, int ldw, void* C, int ldc, int M, int N, int K,
             const float* bias, const void* residual, int ldr, int act, int swiglu, int out_f32, int force_bn,

@@ -22,12 +22,6 @@
 
 namespace sb {
 
-int make_tma_2d(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_rows);
-int make_tma_2d_sw(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_k, int box_rows,
-                   int swizzle_bytes);
-int make_tma_nhwc(CUtensorMap* map, int dtype, const void* base, int N, int H, int W, int C, int box_c, int box_w,
-                  int box_h, int stride, int swizzle_bytes);
-
 struct FmbParams {
   int n_img, H, W, Ho, Wo, Cin, Cmid, Cout, stride;
   int tiles_x, tiles_y;

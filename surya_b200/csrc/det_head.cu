@@ -25,10 +25,6 @@
 
 namespace sb {
 
-int make_tma_2d(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_rows);
-int make_tma_nhwc(CUtensorMap* map, int dtype, const void* base, int N, int H, int W, int C, int box_c, int box_w,
-                  int box_h, int stride, int swizzle_bytes);
-
 constexpr int HEAD_KB = 8;          // k-blocks of 64 channels (K = 512)
 constexpr int HEAD_N = 512;
 

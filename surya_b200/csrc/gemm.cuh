@@ -45,8 +45,8 @@ struct GemmArgs {
   float* am_sum = nullptr;
   int am_ld = 0;
   int store_c = 1;
-  // decode-step kernel (gemm_decode.cu, M <= 256): 0 = off, 1 = on (tile width from its per-shape table unless force_bn).
-  // Same bits as the plain kernel.
+  // decode-step variant of gemm_tn_kernel (M <= 256): 0 = off, 1 = on (tile width from its per-shape table unless
+  // force_bn).  Same bits as the plain kernel.
   int decode = 0;
 };
 // M <= 16 rows: mma.sync kernel without the wgmma pipeline set-up costs (gemm_skinny.cu); gemm_launch routes to it when it applies.
@@ -54,10 +54,6 @@ bool gemm_skinny_ok(const GemmArgs& a);
 int gemm_skinny_launch(const GemmArgs& a, cudaStream_t stream);
 // Tile width gemm_launch will use for an argmax-epilogue launch of this shape (partials per row = ceil(N / width)).
 int gemm_argmax_tile(int M, int N);
-
-// Decode-step kernel: argument check (the combinations it cannot take are refused) and launch.
-int gemm_decode_check(const GemmArgs& a);
-int gemm_decode_launch(const GemmArgs& a, cudaStream_t stream);
 
 // Returns cudaSuccess or an error; sets a message retrievable through sb_last_error().
 int gemm_launch(const GemmArgs& a, cudaStream_t stream);
@@ -72,6 +68,19 @@ int launch_ok();
 long long launch_count();
 void count_launches(long long n);  // kernels replayed through a CUDA graph
 int num_sms();
+
+// TMA descriptors (memoised).  2-D K-major operand map: global [rows, K] with row stride ld (elements), box = box_k x
+// box_rows, swizzle_bytes = 128, 64 or 0.
+int make_tma_2d_sw(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_k, int box_rows,
+                   int swizzle_bytes);
+// The GEMM operand map: box = 64 x box_rows, 128B swizzle.
+inline int make_tma_2d(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_rows) {
+  return make_tma_2d_sw(map, dtype, base, rows, K, ld, 64, box_rows, 128);
+}
+// NHWC activation map for the implicit-GEMM convolution: dims {C, W, H, N}; box {box_c, box_w, box_h, 1} OUTPUT
+// pixels, traversed with `stride` in W and H (boxDim = pixels * stride, elementStrides = stride).
+int make_tma_nhwc(CUtensorMap* map, int dtype, const void* base, int N, int H, int W, int C, int box_c, int box_w,
+                  int box_h, int stride, int swizzle_bytes);
 
 // Launch with the programmatic-stream-serialization attribute (PDL).
 template <typename... P, typename... A>

@@ -37,6 +37,25 @@ struct GemmKParams {
   int store_c;
 };
 
+// Kernel parameters of a dense GEMM launch (gemm_tn_kernel, gemm_splitk_kernel).
+inline GemmKParams gemm_kparams(const GemmArgs& a) {
+  GemmKParams p{};
+  p.M = a.M; p.N = a.N; p.K = a.K;
+  p.C = a.C; p.ldc = a.ldc;
+  p.bias = a.bias;
+  p.residual = a.residual; p.ldr = a.ldr;
+  p.act = a.act; p.swiglu = a.swiglu; p.out_f32 = a.out_f32;
+  p.group_m = 8;
+  p.group_k = a.group_k;
+  p.w_constant = a.w_constant;
+  p.rowscale = a.rowscale;
+  p.ssq_inline = a.ssq_inline;
+  p.ssq_eps = a.ssq_eps;
+  p.ssq_inv_k = 1.0f / static_cast<float>(a.ssq_k > 0 ? a.ssq_k : a.K);
+  p.am_val = a.am_val; p.am_idx = a.am_idx; p.am_sum = a.am_sum; p.am_ld = a.am_ld; p.store_c = a.store_c;
+  return p;
+}
+
 __device__ __forceinline__ float apply_act(float x, int act) {
   switch (act) {
     case ACT_GELU_ERF: return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
@@ -239,7 +258,7 @@ constexpr int EPI_STAGE_BYTES = 32 * 128;                       // per warp: 32 
 constexpr int EPI_ROWSCALE_BYTES = 128 * 4;                     // per-row 1/rms of the tile's 128 rows (folded RMSNorm)
 template <int BN> constexpr int epi_smem_bytes() { return EPI_WARPS * EPI_STAGE_BYTES + BN * 4 + EPI_ROWSCALE_BYTES; }
 
-__device__ __forceinline__ bool epilogue_v2_ok(const GemmKParams& p) {
+__host__ __device__ __forceinline__ bool epilogue_v2_ok(const GemmKParams& p) {
   if (p.out_f32 || (p.ldc & 7) || (p.residual && (p.ldr & 7))) return false;
   if (p.swiglu) return (p.act == ACT_SILU || p.act == ACT_GELU_TANH) && p.N % 16 == 0;
   return p.N % 8 == 0;

@@ -19,8 +19,6 @@
 
 namespace sb {
 
-int make_tma_2d(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_rows);
-
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -245,14 +243,7 @@ static int launch_splitk(const GemmArgs& a, int pk, cudaStream_t stream) {
   if (rc) return rc;
   rc = make_tma_2d(&mb, a.dtype, a.W, a.N, a.K, a.ldw, BN);
   if (rc) return rc;
-  GemmKParams p{};
-  p.M = a.M; p.N = a.N; p.K = a.K;
-  p.C = a.C; p.ldc = a.ldc;
-  p.bias = a.bias;
-  p.residual = a.residual; p.ldr = a.ldr;
-  p.act = a.act; p.swiglu = a.swiglu; p.out_f32 = 0;
-  p.group_m = 1; p.group_k = 0;
-  p.w_constant = a.w_constant;
+  const GemmKParams p = gemm_kparams(a);
   const int m_blocks = (a.M + 127) / 128, n_blocks = (a.N + BN - 1) / BN;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(pk, n_blocks, m_blocks);

@@ -12,9 +12,13 @@
 //     epilogue, which all 8 warps run (tiles wider than 128 columns in two passes).
 // Rounding to the storage type happens exactly where eager PyTorch has an op boundary (after the
 // Linear, after the activation, after the residual add) so results track the reference path.
+//
+// DECODE = true is the recognition decode step's variant (GemmArgs::decode, M <= 256 rows against a large weight matrix):
+// only the single-pass 16-bit staged epilogue, no grouped mode and no fallback epilogue (epilogue_chunk, a __noinline__
+// call).  Without them ptxas gives it no stack frame and, at BN = 128, no spills, and the decode GEMMs run faster
+// (DESIGN.md §5).  Both variants give the same bits.
 #include "gemm.cuh"
 
-#include <mutex>
 #include <string>
 #include <unordered_map>
 #include "gemm_epilogue.cuh"
@@ -37,13 +41,14 @@ __device__ __forceinline__ void tile_coords(int tile, int m_blocks, int n_blocks
   nb = r / gsz;
 }
 
-template <typename T, int BN, int STAGES>
+template <typename T, int BN, int STAGES, bool DECODE>
 __global__ void __launch_bounds__(384, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                const GemmKParams p) {
   constexpr int BM = 128, BK = 64;
   constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int AC = acc_cols<BN>();
+  static_assert(!DECODE || BN <= ACC_MAX_COLS, "the decode variant takes single-pass epilogue tiles only");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // array + offset keeps the shared address space (STS / LDS, not generic ST / LD)
@@ -81,7 +86,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       int early = 0;
       if (p.w_constant && static_cast<int>(blockIdx.x) < num_tiles) {
         int mb, nb;
-        tile_coords(blockIdx.x, m_blocks, n_blocks, p.group_m, mb, nb);
+        if constexpr (DECODE) { mb = static_cast<int>(blockIdx.x) % m_blocks; nb = static_cast<int>(blockIdx.x) / m_blocks; }
+        else tile_coords(blockIdx.x, m_blocks, n_blocks, p.group_m, mb, nb);
         early = k_blocks < STAGES ? k_blocks : STAGES;
         for (int kb = 0; kb < early; ++kb) {
           uint8_t* sa = smem + kb * STAGE_BYTES;
@@ -91,19 +97,26 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       }
       pdl_wait();
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        // The decode variant runs both m-blocks of a weight tile back to back.  At M <= 256 (at most two m-blocks) that is
+        // the order tile_coords gives with group_m = 8, so both variants give the same bits.
         int mb, nb;
-        tile_coords(tile, m_blocks, n_blocks, p.group_m, mb, nb);
+        if constexpr (DECODE) { mb = tile % m_blocks; nb = tile / m_blocks; }
+        else tile_coords(tile, m_blocks, n_blocks, p.group_m, mb, nb);
         for (int kb = 0; kb < k_blocks; ++kb) {
           uint8_t* sa = smem + s * STAGE_BYTES;
           uint8_t* sbp = sa + A_BYTES;
-          if (tile == static_cast<int>(blockIdx.x) && kb < early) {
-            tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + nb * p.group_k, mb * BM);   // B already in flight
-          } else {
+          // B of the first tile's first stages was requested before pdl_wait.  The plain variant requests a stage's A tile
+          // before its B tile, the decode variant after it: one order for both was slower on H100 for prefill or for the
+          // decode step, whichever it did not come from (DESIGN.md §5).  Grouped mode: A columns of this n-block's group.
+          const bool b_in_flight = tile == static_cast<int>(blockIdx.x) && kb < early;
+          if (!DECODE && b_in_flight) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + nb * p.group_k, mb * BM);
+          if (!b_in_flight) {
             mbar_wait(&empty_bar[s], ph ^ 1);
             mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-            tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + nb * p.group_k, mb * BM);
+            if (!DECODE) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + nb * p.group_k, mb * BM);
             tma_load_2d(sbp, &tma_b, &full_bar[s], kb * BK, nb * BN);
           }
+          if (DECODE) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK, mb * BM);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
@@ -121,12 +134,13 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     int s = 0;
     uint32_t ph = 0;
     const bool vec_ok = (p.ldc % 8 == 0) && (!p.residual || p.ldr % 8 == 0);
-    const bool v2 = epilogue_v2_ok(p);
+    const bool v2 = DECODE || epilogue_v2_ok(p);   // the host refuses decode launches the staged epilogue cannot take
     const AccRow acc(acc_s, q * 32 + lane, AC);
     float d[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int mb, nb;
-      tile_coords(tile, m_blocks, n_blocks, p.group_m, mb, nb);
+      if constexpr (DECODE) { mb = tile % m_blocks; nb = tile / m_blocks; }
+      else tile_coords(tile, m_blocks, n_blocks, p.group_m, mb, nb);
       if (v2) {
         asm volatile("bar.sync 1, 256;" ::: "memory");   // all epilogue warps are done with the previous tile's bias
         epilogue_stage_bias<BN>(p, sbias, epi_tid, nb * BN);
@@ -255,30 +269,6 @@ static CUresult encode_tiled_cached(CUtensorMap* map, CUtensorMapDataType dt, in
   return r;
 }
 
-// 2-D K-major operand map: global [rows, K] with row stride ld (elements); box = 64 x box_rows; 128B swizzle.
-int make_tma_2d(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) {
-    set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-    return -1;
-  }
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (static_cast<size_t>(ld) * 2) % 16 != 0) {
-    set_error("TMA operand must be 16B aligned with a 16B-multiple row pitch (ptr=%p ld=%d)", base, ld);
-    return -2;
-  }
-  cuuint64_t dims[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 2};
-  cuuint32_t box[2] = {64, static_cast<cuuint32_t>(box_rows)};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = encode_tiled_cached(map, dtype == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base,
-                                   dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed: %d (rows=%d K=%d ld=%d box_rows=%d)", (int)r, rows, K, ld, box_rows);
-    return -3;
-  }
-  return 0;
-}
-
 int make_tma_2d_sw(CUtensorMap* map, int dtype, const void* base, int rows, int K, int ld, int box_k, int box_rows,
                    int swizzle_bytes) {
   EncodeTiledFn fn = get_encode_fn();
@@ -295,12 +285,13 @@ int make_tma_2d_sw(CUtensorMap* map, int dtype, const void* base, int rows, int 
                                    dims, strides, box, estr,
                                    swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                                         : (swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE));
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(2d) failed: %d", (int)r); return -3; }
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled(2d) failed: %d (rows=%d K=%d ld=%d box=%dx%d)", (int)r, rows, K, ld, box_k, box_rows);
+    return -3;
+  }
   return 0;
 }
 
-// NHWC activation map for the implicit-GEMM convolution: dims {C, W, H, N}; box {box_c, box_w, box_h, 1} OUTPUT
-// pixels, traversed with `stride` in W and H (boxDim = pixels * stride, elementStrides = stride).
 int make_tma_nhwc(CUtensorMap* map, int dtype, const void* base, int N, int H, int W, int C, int box_c, int box_w,
                   int box_h, int stride, int swizzle_bytes) {
   EncodeTiledFn fn = get_encode_fn();
@@ -332,12 +323,12 @@ template <int BN, int STAGES> constexpr size_t gemm_smem_bytes() {
   return STAGES * (128 * 64 * 2 + BN * 64 * 2) + 1024 /*align slack*/ + 256 /*barriers*/ + acc_smem_bytes<BN>() + epi_smem_bytes<BN>();
 }
 
-template <typename T, int BN, int STAGES>
+template <typename T, int BN, int STAGES, bool DECODE>
 static int launch_cfg(const GemmArgs& a, cudaStream_t stream) {
   constexpr size_t SMEM = gemm_smem_bytes<BN, STAGES>();
   static_assert(SMEM <= SMEM_LIMIT, "GEMM tile does not fit in shared memory");
   static bool attr_set = false;
-  auto kern = gemm_tn_kernel<T, BN, STAGES>;
+  auto kern = gemm_tn_kernel<T, BN, STAGES, DECODE>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
     if (e != cudaSuccess) {
@@ -351,20 +342,7 @@ static int launch_cfg(const GemmArgs& a, cudaStream_t stream) {
   if (rc) return rc;
   rc = make_tma_2d(&mb, a.dtype, a.W, a.N, a.K, a.ldw, BN);  // grouped: W is [N, K] with K = padded per-group depth
   if (rc) return rc;
-  GemmKParams p{};
-  p.M = a.M; p.N = a.N; p.K = a.K;
-  p.C = a.C; p.ldc = a.ldc;
-  p.bias = a.bias;
-  p.residual = a.residual; p.ldr = a.ldr;
-  p.act = a.act; p.swiglu = a.swiglu; p.out_f32 = a.out_f32;
-  p.group_m = 8;
-  p.group_k = a.group_k;
-  p.w_constant = a.w_constant;
-  p.rowscale = a.rowscale;
-  p.ssq_inline = a.ssq_inline;
-  p.ssq_eps = a.ssq_eps;
-  p.ssq_inv_k = 1.0f / static_cast<float>(a.ssq_k > 0 ? a.ssq_k : a.K);
-  p.am_val = a.am_val; p.am_idx = a.am_idx; p.am_sum = a.am_sum; p.am_ld = a.am_ld; p.store_c = a.store_c;
+  const GemmKParams p = gemm_kparams(a);
   int m_blocks = (a.M + 127) / 128, n_blocks = (a.N + BN - 1) / BN;
   int tiles = m_blocks * n_blocks;
   int grid = tiles < num_sms() ? tiles : num_sms();
@@ -372,8 +350,31 @@ static int launch_cfg(const GemmArgs& a, cudaStream_t stream) {
   return launch_ok();
 }
 
+// Ring stages per tile width: the most that fit beside the accumulator tile and the epilogue staging.  The decode variant
+// takes the single-pass widths only.
+template <typename T, bool DECODE>
+static int launch_bn(const GemmArgs& a, int bn, cudaStream_t stream) {
+  switch (bn) {
+    case 128: return launch_cfg<T, 128, 4, DECODE>(a, stream);
+    case 64: return launch_cfg<T, 64, 6, DECODE>(a, stream);
+    case 32: return launch_cfg<T, 32, 8, DECODE>(a, stream);
+  }
+  if constexpr (!DECODE) {
+    if (bn == 256) return launch_cfg<T, 256, 2, false>(a, stream);
+    if (bn == 96) return launch_cfg<T, 96, 5, false>(a, stream);
+  }
+  set_error("unsupported BN %d", bn);
+  return -12;
+}
+
 template <typename T>
 static int launch_typed(const GemmArgs& a, cudaStream_t stream) {
+  if (a.decode) {
+    // Tile width per decode shape, measured on H100 (DESIGN.md §5): 32 for the 1280- / 1920-wide qkv and o projections, 128
+    // for gate/up; the argmax epilogue keeps gemm_argmax_tile's width, which sized the caller's partial buffers.
+    const int bn = a.force_bn ? a.force_bn : a.am_val ? gemm_argmax_tile(a.M, a.N) : a.N >= 4096 ? 128 : 32;
+    return launch_bn<T, true>(a, bn, stream);
+  }
   int bn = a.force_bn;
   if (bn >= 1000) return gemm_splitk_launch(a, bn / 1000, bn % 1000, stream);   // forced split-K: 1000 * pk + BN
   if (bn == 0 && a.allow_splitk && !a.rowscale && !a.ssq_inline && !a.am_val) {
@@ -411,14 +412,7 @@ static int launch_typed(const GemmArgs& a, cudaStream_t stream) {
   }
   if (a.am_val && a.force_bn == 0) bn = gemm_argmax_tile(a.M, a.N);   // the caller sized its partial buffers with this
   if (a.group_k) bn = a.group_n;  // one n-block per channel group
-  switch (bn) {
-    case 256: return launch_cfg<T, 256, 2>(a, stream);
-    case 128: return launch_cfg<T, 128, 4>(a, stream);
-    case 96: return launch_cfg<T, 96, 5>(a, stream);
-    case 64: return launch_cfg<T, 64, 6>(a, stream);
-    case 32: return launch_cfg<T, 32, 8>(a, stream);
-    default: set_error("unsupported BN %d", bn); return -12;
-  }
+  return launch_bn<T, false>(a, bn, stream);
 }
 
 int gemm_argmax_tile(int M, int N) {
@@ -440,11 +434,10 @@ int gemm_launch(const GemmArgs& a, cudaStream_t stream) {
   }
   if (a.swiglu && a.residual) { set_error("gemm: the swiglu epilogue takes no residual"); return -20; }
   if (a.out_f32 && (a.residual || a.swiglu)) { set_error("gemm: out_f32 takes no residual and no swiglu"); return -20; }
+  const bool staged = epilogue_v2_ok(gemm_kparams(a));   // the kernels' own rule for the 16-bit staged epilogue
   if (a.rowscale || a.ssq_inline || a.am_val) {
     // these ride on the staged 16-bit epilogue only (and on the plain kernel: split-K would change who owns a row's columns)
-    const bool v2 = !a.out_f32 && a.ldc % 8 == 0 && (!a.residual || a.ldr % 8 == 0) &&
-                    (a.swiglu ? ((a.act == ACT_SILU || a.act == ACT_GELU_TANH) && a.N % 16 == 0) : a.N % 8 == 0);
-    if (!v2 || a.group_k || a.force_bn >= 1000) {
+    if (!staged || a.group_k || a.force_bn >= 1000) {
       set_error("gemm: rowscale / ssq_inline / argmax epilogues need the 16-bit staged epilogue (N %% 8 == 0, 16-byte pitches), "
                 "no grouped or split-K mode");
       return -15;
@@ -459,11 +452,24 @@ int gemm_launch(const GemmArgs& a, cudaStream_t stream) {
   }
   if (a.dtype != DT_BF16 && a.dtype != DT_F16) { set_error("unsupported dtype %d", a.dtype); return -14; }
   if (a.decode) {
-    const int rc = gemm_decode_check(a);
-    if (rc) return rc;
+    if (a.decode != 1) {
+      set_error("gemm: decode must be 0 or 1 (got %d)", a.decode);
+      return -21;
+    }
+    if (a.M > 256 || a.out_f32 || a.group_k || a.force_bn >= 1000) {
+      set_error("gemm: the decode kernel takes M <= 256 (got %d), 16-bit output, no grouped or forced split-K mode", a.M);
+      return -21;
+    }
+    if (a.force_bn != 0 && a.force_bn != 32 && a.force_bn != 64 && a.force_bn != 128) {
+      set_error("gemm: the decode kernel's tile width is 32, 64 or 128 (got %d)", a.force_bn);
+      return -21;
+    }
+    if (!staged) {
+      set_error("gemm: the decode kernel needs the 16-bit staged epilogue (N %% 8 == 0, N %% 16 == 0 with swiglu, 16-byte pitches)");
+      return -21;
+    }
   }
   if (gemm_skinny_ok(a)) return gemm_skinny_launch(a, stream);
-  if (a.decode) return gemm_decode_launch(a, stream);
   if (a.dtype == DT_BF16) return launch_typed<__nv_bfloat16>(a, stream);
   return launch_typed<__half>(a, stream);
 }

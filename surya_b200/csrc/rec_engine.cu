@@ -165,7 +165,7 @@ static int run_heads(sb_rec_engine* e, void* hidden, int rows, const HeadOut& o,
   a.rowscale = e->rs;
   a.am_val = e->am_val; a.am_idx = e->am_idx; a.am_sum = e->am_sum; a.am_ld = e->am_ld;
   a.store_c = o.logits ? 1 : 0;
-  a.decode = rows <= 256 ? 1 : 0;   // decode-step kernel (gemm_decode.cu): same bits, faster at these shapes
+  a.decode = rows <= 256 ? 1 : 0;   // decode-step GEMM variant: same bits, faster at these shapes
   CK(gemm_launch(a, st));
   DecodeTailArgs t;
   t.rows = rows;
@@ -239,7 +239,7 @@ static int run_decode_step(sb_rec_engine* e, const long long* ids, const int* sl
   const int Q = (nh + 2 * nkv) * hd;
   const int dt = c.dtype;
   void* x = e->x;
-  // qkv, o and gate/up take the decode-step kernel (gemm_decode.cu, same bits); the down projection keeps split-K
+  // qkv, o and gate/up take the decode-step GEMM variant (same bits); the down projection keeps split-K
   const int dec = B <= 256 ? 1 : 0;
   if (ids) CK(embed_rows(dt, ids, e->W(SB_RW_EMBED), x, D, B, D, st));
   for (int l = 0; l < c.dec_layers; ++l) {

@@ -35,7 +35,7 @@ def gemm(a, w, bias=None, residual=None, act="none", swiglu=False, out=None, out
     rms_eps / rowscale: RMSNorm folded into the GEMM (sb_gemm_rmsnorm): w already carries the norm weight, rows are scaled by
     `rowscale` (fp32 [M]) or by 1/rms computed in the kernel with rms_eps.  argmax: dict filled with the per-tile partials
     (val, idx, sum) of the online argmax epilogue; argmax_only skips writing the logits.
-    decode=1: the decode-step kernel for M <= 256 (sb_gemm); same bits as the plain kernel."""
+    decode=1: the GEMM kernel's decode-step variant for M <= 256 (sb_gemm); same bits as the plain variant."""
     if splitk and force_bn == 0:
         force_bn = -1
     lib = _lib.load()

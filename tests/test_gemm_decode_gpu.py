@@ -1,11 +1,12 @@
-"""The decode-step GEMM kernel (gemm_decode.cu) against the plain kernel (GPU).
+"""The decode-step variant of the GEMM kernel against the plain variant (GPU).
 
-gemm_decode_kernel must give the bits of gemm_tn_kernel at any tile width: every output element is the same per-k-block
-partial sums added in k order.  Each case runs both kernels on the same operands and compares them with torch.equal, in the
-four configurations the recognition decode step launches (qkv with the folded RMSNorm and a bias, o-proj with an in-place
-residual, gate/up with SwiGLU and the folded norm, lm_head with row scales and the argmax partials), at row counts on both
-sides of the 128-row tile, at every tile width the kernel takes and at its own table's choice, with k-block counts of 1, 2,
-odd, even and with a partial last block, and with more tiles than SMs (each CTA runs several).
+gemm_tn_kernel<T, BN, STAGES, true> must give the bits of gemm_tn_kernel<T, BN, STAGES, false> at any tile width: every
+output element is the same per-k-block partial sums added in k order.  Each case runs both instantiations on the same
+operands and compares them with torch.equal, in the four configurations the recognition decode step launches (qkv with the
+folded RMSNorm and a bias, o-proj with an in-place residual, gate/up with SwiGLU and the folded norm, lm_head with row scales
+and the argmax partials), at row counts on both sides of the 128-row tile, at every tile width the decode variant takes and
+at its own table's choice, with k-block counts of 1, 2, odd, even and with a partial last block, and with more tiles than SMs
+(each CTA runs several).
 Operands are windows of NaN-filled buffers and outputs windows of sentinel-filled ones, as in test_gemm_contract_gpu.py."""
 import pytest
 import torch

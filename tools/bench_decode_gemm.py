@@ -1,7 +1,7 @@
-"""Micro-benchmark (GPU box): the recognition decode step's GEMMs that take the decode kernel (gemm_decode.cu), at their real
+"""Micro-benchmark (GPU box): the recognition decode step's GEMMs that take gemm_tn_kernel's decode variant, at their real
 shapes (SYN-REC, B = 256, bf16), each timed INSIDE a CUDA graph of back-to-back launches with the weights rotated over more
-than L2 holds (as tools/bench_decode_parts.py does): gemm_tn_kernel ("plain"; "plain heuristic" = its own tile width) and the
-decode kernel (decode=1; "decode table" = its own tile width) at every tile width the decode kernel takes.
+than L2 holds (as tools/bench_decode_parts.py does): the plain variant ("plain"; "plain heuristic" = its own tile width) and
+the decode variant (decode=1; "decode table" = its own tile width) at every tile width the decode variant takes.
 
 Prints us per launch and the algorithmic GB/s ((A + W + C (+ residual)) bytes / time), then a markdown table."""
 import sys
