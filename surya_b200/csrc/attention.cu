@@ -274,20 +274,66 @@ struct DecodeKParams {
   float scale;
 };
 
+// One CTA of 128 threads per (batch row, KV head).  The cache rows 0 .. pos-1 of a (slot, KV head) are contiguous, so they
+// stream through a ring of DEC_STAGES shared-memory chunks of DEC_CK keys with 1-D bulk copies (cp.async.bulk completing on
+// one mbarrier per stage): K chunks 0 .. nc-1, then V chunks 0 .. nc-1, nc = ceil(n_keys / DEC_CK).  Thread 0 requests the
+// first DEC_STAGES chunks right after griddepcontrol.wait and refills a stage as soon as the CTA has consumed it, so the
+// loads run under the RoPE step, the scores and the softmax, and the first V chunks are in flight before P.V starts.  The
+// appended row (key pos) is never read back from global memory: the RoPE step keeps a copy in shared memory.  The ring holds
+// DEC_STAGES * DEC_CK keys (20 KB at HD = 80), not the whole slab, so residency does not depend on the key count.
+//
+// Summation trees.  They fix the output bits and do not depend on how the work is spread over the threads
+// (VPR = HD / 8, NKG = 128 / VPR):
+//  - score s[g][j] = (fp32 chain acc = fmaf(q[g][x], k[j][x], acc), x = 0 .. HD-1 ascending, from 0.f) * scale.  The
+//    16-bit products are exact in fp32, so q lives in shared memory as fp32, converted once;
+//  - m_g = max over j of s[g][j] (order-free);
+//  - l_g: 128 lanes t each sum __expf(s[g][j] - m_g) over j = t (mod 128) ascending from 0.f, then the xor butterfly 16, 8,
+//    4, 2, 1 inside each warp, then ((w0 + w1) + w2) + w3;
+//  - p[g][j] = rnd_T(__expf(s[g][j] - m_g)), kept as the fp32 value of the rounded number;
+//  - out[g][d] = rnd_T(o / l_g) with o the sum over kg = 0 .. NKG-1, in order from 0.f, of the fp32 chains
+//    fmaf(p[g][j], v[j][d], acc) over j = kg, kg + NKG, kg + 2 NKG, ... ascending from 0.f;
+//  - RoPE: o1 = rnd(rnd(x1 c) + rnd(-x2 s)), o2 = rnd(rnd(x2 c) + rnd(x1 s)), c = rnd(cosf(pos inv_freq)), s likewise.
+constexpr int DEC_CK = 32, DEC_STAGES = 4;
+
 template <typename T, int HD, int G>
-__global__ void __launch_bounds__(128) decode_attn_kernel(const DecodeKParams p) {
-  constexpr int HALF = HD / 2, VPR = HD / 8, NKG = 128 / VPR;
-  extern __shared__ __align__(16) uint8_t smem_dec[];
-  T* q_t = reinterpret_cast<T*>(smem_dec);                  // [G][HD] rotated queries (in T; the first G*HD floats' worth of space)
-  float* red = reinterpret_cast<float*>(smem_dec) + G * HD;  // [NKG][G][HD]
-  float* sc = red + NKG * G * HD;                           // [G][s_max]
+struct DecodeSmem {
+  static constexpr int VPR = HD / 8, NKG = 128 / VPR, QS = HD + 4;  // QS: q row pitch in floats (conflict-free float4 reads)
+  static constexpr int CHUNK = DEC_CK * HD * static_cast<int>(sizeof(T));
+  static constexpr int RED = NKG * G * HD * 4;
+  // [DEC_STAGES][DEC_CK][HD] T ring, reused as red [NKG][G][HD] fp32 once every chunk is consumed
+  static constexpr int RING = DEC_STAGES * CHUNK > RED ? DEC_STAGES * CHUNK : RED;
+  static constexpr int Q_OFF = RING;                                              // [G][QS] fp32 rotated queries
+  static constexpr int KN_OFF = Q_OFF + G * QS * 4;                               // [HD] T appended K row (after RoPE)
+  static constexpr int VN_OFF = KN_OFF + HD * static_cast<int>(sizeof(T));        // [HD] T appended V row
+  static constexpr int BAR_OFF = VN_OFF + HD * static_cast<int>(sizeof(T));       // [DEC_STAGES] mbarriers
+  static constexpr int SC_OFF = BAR_OFF + DEC_STAGES * 8;                         // [G][s_max + 1] fp32 scores, then p
+  static_assert(CHUNK % 16 == 0 && RING % 16 == 0 && KN_OFF % 16 == 0 && VN_OFF % 16 == 0 && BAR_OFF % 8 == 0, "alignment");
+  static size_t bytes(int s_max) { return SC_OFF + static_cast<size_t>(G) * (s_max + 1) * sizeof(float); }
+};
+
+template <typename T, int HD, int G>
+__global__ void __launch_bounds__(128, G <= 4 ? 8 : 1) decode_attn_kernel(const DecodeKParams p) {
+  using L = DecodeSmem<T, HD, G>;
+  constexpr int HALF = HD / 2, VPR = L::VPR, NKG = L::NKG, QS = L::QS;
+  extern __shared__ __align__(128) uint8_t smem_dec[];
+  uint8_t* ring = smem_dec;
+  float* red = reinterpret_cast<float*>(smem_dec);
+  float* qf = reinterpret_cast<float*>(smem_dec + L::Q_OFF);
+  T* knew = reinterpret_cast<T*>(smem_dec + L::KN_OFF);
+  T* vnew = reinterpret_cast<T*>(smem_dec + L::VN_OFF);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_dec + L::BAR_OFF);
+  float* sc = reinterpret_cast<float*>(smem_dec + L::SC_OFF);
   __shared__ float s_red[4][G];
   __shared__ float s_max_g[G], s_sum_g[G];
 
   pdl_trigger();
-  pdl_wait();
-  const int b = blockIdx.x, kvh = blockIdx.y;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (tid == 0) {
+    for (int i = 0; i < DEC_STAGES; ++i) mbar_init(&full[i], 1);
+    mbar_fence_init();
+  }
+  pdl_wait();  // every global read below (qkv, slot, pos and the cache rows) comes after it
+  const int b = blockIdx.x, kvh = blockIdx.y;
   const int slot = p.slot[b];
   const int pos = p.pos[b];
   const int n_keys = pos + 1;
@@ -301,8 +347,22 @@ __global__ void __launch_bounds__(128) decode_attn_kernel(const DecodeKParams p)
   const T* row = reinterpret_cast<const T*>(p.qkv) + static_cast<size_t>(b) * p.ld;
   T* kc = reinterpret_cast<T*>(p.kcache) + (static_cast<size_t>(slot) * p.n_kv_heads + kvh) * p.s_max * HD;
   T* vc = reinterpret_cast<T*>(p.vcache) + (static_cast<size_t>(slot) * p.n_kv_heads + kvh) * p.s_max * HD;
+  const int sp = p.s_max + 1;  // score row pitch: the G rows of a key fall in different banks
+  const int nc = (n_keys + DEC_CK - 1) / DEC_CK;
 
-  // ---- RoPE on the G query heads and the new key; append k, v
+  // stream step s < 2 nc loads K chunk s (s < nc) or V chunk s - nc into stage s % DEC_STAGES, phase (s / DEC_STAGES) & 1;
+  // chunk c holds cache rows [c DEC_CK, min((c + 1) DEC_CK, pos)), none when it only holds the appended row
+  auto issue = [&](int s) {
+    const int c = s < nc ? s : s - nc;
+    const uint32_t bytes = static_cast<uint32_t>(min(DEC_CK, pos - c * DEC_CK)) * HD * sizeof(T);
+    uint64_t* bar = &full[s % DEC_STAGES];
+    mbar_expect_tx(bar, bytes);
+    if (bytes) bulk_load(ring + (s % DEC_STAGES) * L::CHUNK, (s < nc ? kc : vc) + static_cast<size_t>(c) * DEC_CK * HD, bytes, bar);
+  };
+  if (tid == 0)
+    for (int s = 0; s < min(DEC_STAGES, 2 * nc); ++s) issue(s);
+
+  // ---- RoPE on the G query heads and the new key; append k, v (and keep them for the key pos)
   for (int idx = tid; idx < (G + 1) * HALF; idx += 128) {
     int hh = idx / HALF, i = idx % HALF;
     const T* src = (hh < G) ? row + (kvh * G + hh) * HD : row + (p.n_heads + kvh) * HD;
@@ -312,56 +372,63 @@ __global__ void __launch_bounds__(128) decode_attn_kernel(const DecodeKParams p)
     float o1 = rnd<T>(rnd<T>(x1 * c) + rnd<T>(-x2 * s));
     float o2 = rnd<T>(rnd<T>(x2 * c) + rnd<T>(x1 * s));
     if (hh < G) {
-      q_t[hh * HD + i] = from_f<T>(o1);          // exactly representable: o1 / o2 are already rounded to T
-      q_t[hh * HD + i + HALF] = from_f<T>(o2);
+      qf[hh * QS + i] = o1;  // o1 / o2 are already rounded to T
+      qf[hh * QS + i + HALF] = o2;
     } else {
-      kc[static_cast<size_t>(pos) * HD + i] = from_f<T>(o1);
-      kc[static_cast<size_t>(pos) * HD + i + HALF] = from_f<T>(o2);
+      const T k1 = from_f<T>(o1), k2 = from_f<T>(o2);
+      kc[static_cast<size_t>(pos) * HD + i] = k1;
+      kc[static_cast<size_t>(pos) * HD + i + HALF] = k2;
+      knew[i] = k1;
+      knew[i + HALF] = k2;
     }
   }
   {
     const T* vsrc = row + (p.n_heads + p.n_kv_heads + kvh) * HD;
-    for (int i = tid; i < HD; i += 128) vc[static_cast<size_t>(pos) * HD + i] = vsrc[i];
+    for (int i = tid; i < HD; i += 128) {
+      const T v = vsrc[i];
+      vc[static_cast<size_t>(pos) * HD + i] = v;
+      vnew[i] = v;
+    }
   }
   __syncthreads();
 
-  // ---- scores: one key per thread
-  float tmax[G];
+  // ---- scores, one K chunk at a time: item it = (key it / G of the chunk, head it % G); 128 % G == 0, so a thread's head is fixed
+  const int gs = tid % G;
+  const float* qg = qf + gs * QS;
+  float tmax = -INFINITY;
+  for (int c = 0; c < nc; ++c) {
+    const int st = c % DEC_STAGES;
+    mbar_wait(&full[st], (c / DEC_STAGES) & 1);
+    const T* kst = reinterpret_cast<const T*>(ring + st * L::CHUNK);
+    const int c0 = c * DEC_CK, ck = min(DEC_CK, n_keys - c0);
+    for (int it = tid; it < ck * G; it += 128) {
+      const int jl = it / G, j = c0 + jl;
+      const uint4* kr = reinterpret_cast<const uint4*>(j == pos ? knew : kst + jl * HD);
+      float acc = 0.f;
 #pragma unroll
-  for (int gq = 0; gq < G; ++gq) tmax[gq] = -INFINITY;
-#pragma unroll 2
-  for (int j = tid; j < n_keys; j += 128) {
-    const uint4* kr = reinterpret_cast<const uint4*>(kc + static_cast<size_t>(j) * HD);
-    float acc[G];
-#pragma unroll
-    for (int gq = 0; gq < G; ++gq) acc[gq] = 0.f;
-#pragma unroll
-    for (int c = 0; c < VPR; ++c) {
-      uint4 u = kr[c];
-      const T* e = reinterpret_cast<const T*>(&u);
-      const unsigned short* kb = reinterpret_cast<const unsigned short*>(e);
-#pragma unroll
-      for (int gq = 0; gq < G; ++gq) {
-        // one 16-byte broadcast read of 8 q values (kept in T: they are rounded to T anyway) and 8 mixed-precision FMAs
-        // (FHFMA: 16-bit operands, fp32 accumulate, no conversion instructions) — bit-identical to fmaf(float(q), float(k), acc)
-        const uint4 qv = *reinterpret_cast<const uint4*>(q_t + gq * HD + c * 8);
-        const unsigned short* qb = reinterpret_cast<const unsigned short*>(&qv);
-#pragma unroll
-        for (int x = 0; x < 8; ++x) acc[gq] = fma16<T>(qb[x], kb[x], acc[gq]);
+      for (int c8 = 0; c8 < VPR; ++c8) {
+        const uint4 u = kr[c8];
+        const T* e = reinterpret_cast<const T*>(&u);
+        const float4 qa = reinterpret_cast<const float4*>(qg + c8 * 8)[0];
+        const float4 qb = reinterpret_cast<const float4*>(qg + c8 * 8)[1];
+        acc = fmaf(qa.x, to_f<T>(e[0]), acc);
+        acc = fmaf(qa.y, to_f<T>(e[1]), acc);
+        acc = fmaf(qa.z, to_f<T>(e[2]), acc);
+        acc = fmaf(qa.w, to_f<T>(e[3]), acc);
+        acc = fmaf(qb.x, to_f<T>(e[4]), acc);
+        acc = fmaf(qb.y, to_f<T>(e[5]), acc);
+        acc = fmaf(qb.z, to_f<T>(e[6]), acc);
+        acc = fmaf(qb.w, to_f<T>(e[7]), acc);
       }
+      const float sv = acc * p.scale;
+      sc[gs * sp + j] = sv;
+      tmax = fmaxf(tmax, sv);
     }
-#pragma unroll
-    for (int gq = 0; gq < G; ++gq) {
-      float sv = acc[gq] * p.scale;
-      sc[gq * p.s_max + j] = sv;
-      tmax[gq] = fmaxf(tmax[gq], sv);
-    }
+    __syncthreads();  // stage st consumed
+    if (tid == 0 && c + DEC_STAGES < 2 * nc) issue(c + DEC_STAGES);
   }
-#pragma unroll
-  for (int gq = 0; gq < G; ++gq) {
-    float m = warp_max(tmax[gq]);
-    if (lane == 0) s_red[warp][gq] = m;
-  }
+  for (int o = 16; o >= G; o >>= 1) tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, o));
+  if (lane < G) s_red[warp][lane] = tmax;
   __syncthreads();
   if (tid < G) s_max_g[tid] = fmaxf(fmaxf(s_red[0][tid], s_red[1][tid]), fmaxf(s_red[2][tid], s_red[3][tid]));
   __syncthreads();
@@ -371,9 +438,9 @@ __global__ void __launch_bounds__(128) decode_attn_kernel(const DecodeKParams p)
   for (int j = tid; j < n_keys; j += 128) {
 #pragma unroll
     for (int gq = 0; gq < G; ++gq) {
-      float pv = __expf(sc[gq * p.s_max + j] - s_max_g[gq]);
+      float pv = __expf(sc[gq * sp + j] - s_max_g[gq]);
       tsum[gq] += pv;
-      sc[gq * p.s_max + j] = rnd<T>(pv);
+      sc[gq * sp + j] = rnd<T>(pv);
     }
   }
 #pragma unroll
@@ -385,38 +452,39 @@ __global__ void __launch_bounds__(128) decode_attn_kernel(const DecodeKParams p)
   if (tid < G) s_sum_g[tid] = s_red[0][tid] + s_red[1][tid] + s_red[2][tid] + s_red[3][tid];
   __syncthreads();
 
-  // ---- O = P V : thread = (key group, 8-wide dim chunk)
+  // ---- O = P V, one V chunk at a time: thread = (key group kg, 8-wide dim chunk); jn walks j = kg (mod NKG) across the chunks
   const int chunk = tid % VPR, kg = tid / VPR;
-  if (kg < NKG) {
-    float acc[G][8];
+  float acc[G][8];
 #pragma unroll
-    for (int gq = 0; gq < G; ++gq)
+  for (int gq = 0; gq < G; ++gq)
 #pragma unroll
-      for (int x = 0; x < 8; ++x) acc[gq][x] = 0.f;
-    // keys in batches of PVU with every V load of the batch issued before the first use: the loop is a DRAM-latency chain
-    // otherwise (one dependent 16-byte load per iteration).  (A 256-thread variant that prefetched all K / V rows into
-    // registers up front was 18 % slower end to end: it halves the number of resident CTAs.)
-    constexpr int PVU = 4;
-    for (int j0 = kg; j0 < n_keys; j0 += NKG * PVU) {
-      uint4 u[PVU];
+    for (int x = 0; x < 8; ++x) acc[gq][x] = 0.f;
+  int jn = kg;
+  for (int c = 0; c < nc; ++c) {
+    const int s = nc + c, st = s % DEC_STAGES;
+    mbar_wait(&full[st], (s / DEC_STAGES) & 1);
+    if (kg < NKG) {
+      const T* vst = reinterpret_cast<const T*>(ring + st * L::CHUNK);
+      const int c0 = c * DEC_CK, c1 = min(c0 + DEC_CK, n_keys);
+      for (; jn < c1; jn += NKG) {
+        const uint4 u = reinterpret_cast<const uint4*>(jn == pos ? vnew : vst + (jn - c0) * HD)[chunk];
+        const T* e = reinterpret_cast<const T*>(&u);
+        float vf[8];
 #pragma unroll
-      for (int t = 0; t < PVU; ++t) {
-        const int j = j0 + t * NKG;
-        u[t] = j < n_keys ? *reinterpret_cast<const uint4*>(vc + static_cast<size_t>(j) * HD + chunk * 8) : make_uint4(0u, 0u, 0u, 0u);
-      }
-#pragma unroll
-      for (int t = 0; t < PVU; ++t) {
-        const int j = j0 + t * NKG;
-        if (j >= n_keys) break;
-        const unsigned short* vb = reinterpret_cast<const unsigned short*>(&u[t]);
+        for (int x = 0; x < 8; ++x) vf[x] = to_f<T>(e[x]);
 #pragma unroll
         for (int gq = 0; gq < G; ++gq) {
-          const unsigned short pb = bits_of<T>(from_f<T>(sc[gq * p.s_max + j]));     // p was rounded to T after the softmax
+          const float pg = sc[gq * sp + jn];
 #pragma unroll
-          for (int x = 0; x < 8; ++x) acc[gq][x] = fma16<T>(pb, vb[x], acc[gq][x]);
+          for (int x = 0; x < 8; ++x) acc[gq][x] = fmaf(pg, vf[x], acc[gq][x]);
         }
       }
     }
+    __syncthreads();  // stage st consumed
+    if (tid == 0 && s + DEC_STAGES < 2 * nc) issue(s + DEC_STAGES);
+  }
+  // every issued chunk has been waited for and consumed: the ring is free for the partials
+  if (kg < NKG) {
 #pragma unroll
     for (int gq = 0; gq < G; ++gq)
 #pragma unroll
@@ -434,9 +502,7 @@ __global__ void __launch_bounds__(128) decode_attn_kernel(const DecodeKParams p)
 
 template <typename T, int HD, int G>
 static int launch_decode(const DecodeAttnArgs& a, cudaStream_t st) {
-  constexpr int NKG = 128 / (HD / 8);
-  size_t smem = (static_cast<size_t>(G) * HD + static_cast<size_t>(NKG) * G * HD + static_cast<size_t>(G) * a.s_max) *
-                sizeof(float);
+  const size_t smem = DecodeSmem<T, HD, G>::bytes(a.s_max);
   auto kern = decode_attn_kernel<T, HD, G>;
   static size_t attr = 0;
   if (smem > 48 * 1024 && smem > attr) {
@@ -482,6 +548,10 @@ int decode_attn(const DecodeAttnArgs& a, cudaStream_t st) {
   if (a.batch <= 0) return 0;
   if (a.n_kv_heads <= 0 || a.n_heads % a.n_kv_heads) {
     set_error("decode_attn: n_heads must be a positive multiple of n_kv_heads"); return -1;
+  }
+  // the cache rows are read with 16-byte bulk copies
+  if ((reinterpret_cast<uintptr_t>(a.kcache) | reinterpret_cast<uintptr_t>(a.vcache)) % 16) {
+    set_error("decode_attn: kcache and vcache must be 16B aligned"); return -1;
   }
   return a.dtype == DT_BF16 ? dispatch_decode<__nv_bfloat16>(a, st) : dispatch_decode<__half>(a, st);
 }

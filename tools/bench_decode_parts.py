@@ -1,6 +1,7 @@
 """Micro-benchmark (GPU box): every kernel of one recognition decode step (SYN-REC, B = 256, bf16) timed INSIDE a CUDA graph of
 back-to-back launches (PDL on, weights rotated over > L2 worth of copies), plus whole decoder-layer sequences, so the step
 time can be attributed.  Writes a markdown table to stdout."""
+import subprocess
 import sys
 from pathlib import Path
 
@@ -13,6 +14,7 @@ DT = torch.bfloat16
 B, D, Q, I2, IP, V = 256, 1280, 1920, 6848, 3424, 65792
 NH, NKV, HD, SMAX = 16, 4, 80, 256
 EPS = 1e-6
+HBM_BPS = 3.35e12  # H100 SXM data sheet
 
 
 def timeit(fn, n=48, reps=5):
@@ -39,8 +41,19 @@ def copies(N, K, cap=24):
     return [torch.randn(N, K, device="cuda").to(DT) * 0.03 for _ in range(n)]
 
 
+def card():
+    """The card's name and power limit: part of every number below."""
+    try:
+        limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
+                               capture_output=True, text=True, check=True).stdout.strip()
+    except (OSError, subprocess.CalledProcessError):
+        limit = "power limit unknown"
+    return f"{torch.cuda.get_device_name(0)}, {limit}"
+
+
 def main():
     rows = []
+    print(f"card: {card()}", flush=True)
 
     def rec(name, us, note=""):
         rows.append((name, us, note))
@@ -86,11 +99,18 @@ def main():
     slot = torch.arange(B, dtype=torch.int32, device="cuda")
     inv = (1.0 / (10000.0 ** (torch.arange(0, HD, 2, device="cuda").float() / HD))).contiguous()
     qk = torch.randn(B, Q, device="cuda").to(DT)
-    for S in (46, 110, 173):
-        pos = torch.full((B,), S, dtype=torch.int32, device="cuda")
+    # KV bytes: every row reads keys 0 .. pos of its KV heads, K and V; the floor is those bytes at the data sheet's 3.35 TB/s
+    def attn_case(name, pos):
         us = timeit(lambda i: ops.decode_attn(qk, kc[i % 24], vc[i % 24], slot, pos, inv, NH, NKV, HD, HD ** -0.5, out=ao))
-        gb = B * NKV * (S + 1) * HD * 2 * 2 / 1e9
-        rec(f"decode_attn S={S}", us, f"{gb / (us * 1e-6):.0f} GB/s of KV")
+        nbytes = NKV * int((pos.long() + 1).sum()) * HD * 2 * 2
+        floor_us = nbytes / HBM_BPS * 1e6
+        rec(name, us, f"{nbytes / 1e3 / us:.0f} GB/s of KV, {us / floor_us:.2f}x the {floor_us:.2f} us floor")
+
+    for S in (46, 110, 173):
+        attn_case(f"decode_attn S={S}", torch.full((B,), S, dtype=torch.int32, device="cuda"))
+    # the benchmark's decode step: s_max = 256 with ragged positions across the 256 rows
+    ragged = torch.randint(46, 173, (B,), generator=torch.Generator().manual_seed(0)).to(device="cuda", dtype=torch.int32)
+    attn_case("decode_attn ragged 46..172", ragged)
 
     # ---- one decoder layer as the engine launches it (5 kernels) and the round-1 sequence (7 kernels)
     pos = torch.full((B,), 110, dtype=torch.int32, device="cuda")
