@@ -3,18 +3,12 @@
 // Stands in for EfficientViTForSemanticSegmentation.forward (surya/detection/model/encoderdecoder.py:725-753):
 // dense 3x3 convs -> conv_wgmma.cu, 1x1 / grouped 1x1 convs -> gemm_wgmma.cu, everything else -> det_ops.cu.
 #include "../../include/surya_b200.h"
-#include "ops.cuh"
+#include "engine.cuh"
 #include "sb_ptx.cuh"
 
 #include <vector>
 
 using namespace sb;
-
-#define CK(x)            \
-  do {                   \
-    int rc_ = (x);       \
-    if (rc_) return rc_; \
-  } while (0)
 
 struct BufDim { int H = 0, W = 0, C = 0; };
 
@@ -26,11 +20,8 @@ struct sb_det_engine {
   std::vector<void*> bufs;
   std::vector<BufDim> dims;
   int max_batch = 0;
-  uint8_t* arena = nullptr;
-  size_t arena_bytes = 0;
+  Arena arena;
 };
-
-static size_t al256(size_t v) { return (v + 255) & ~size_t(255); }
 
 extern "C" {
 
@@ -47,33 +38,22 @@ int sb_det_create(int dtype, const sb_det_op* ops, int n_ops, const void* const*
     if (op.w >= n_weights || op.b >= n_weights) { set_error("sb_det_create: weight index out of range"); delete e; return -2; }
     if (op.dst >= n_bufs) { set_error("sb_det_create: buffer index out of range"); delete e; return -2; }
   }
-  size_t total = 0;
-  for (long long n : e->buf_elems) total += al256(static_cast<size_t>(n) * max_batch * 2);
-  cudaError_t ce = cudaMalloc(&e->arena, total);
+  e->bufs.resize(n_bufs);
+  for (int i = 0; i < n_bufs; ++i) e->arena.add(e->bufs[i], static_cast<size_t>(e->buf_elems[i]) * max_batch * 2);
+  cudaError_t ce = e->arena.alloc();
   if (ce != cudaSuccess) {
-    cudaGetLastError();
-    set_error("sb_det_create: cudaMalloc(%zu MiB) failed: %s", total >> 20, cudaGetErrorString(ce));
+    set_error("sb_det_create: cudaMalloc(%zu MiB) failed: %s", e->arena.bytes() >> 20, cudaGetErrorString(ce));
     delete e;
     return -3;
-  }
-  e->arena_bytes = total;
-  uint8_t* p = e->arena;
-  for (long long n : e->buf_elems) {
-    e->bufs.push_back(p);
-    p += al256(static_cast<size_t>(n) * max_batch * 2);
   }
   e->dims.resize(n_bufs);
   *out = e;
   return 0;
 }
 
-void sb_det_destroy(sb_det_engine* e) {
-  if (!e) return;
-  if (e->arena) cudaFree(e->arena);
-  delete e;
-}
+void sb_det_destroy(sb_det_engine* e) { delete e; }
 
-size_t sb_det_workspace_bytes(const sb_det_engine* e) { return e ? e->arena_bytes : 0; }
+size_t sb_det_workspace_bytes(const sb_det_engine* e) { return e ? e->arena.bytes() : 0; }
 
 int sb_det_forward(sb_det_engine* e, const void* pixel_values, int in_f32, int B, int H, int W, void* logits, void* stream) {
   if (!e) { set_error("sb_det_forward: null engine"); return -1; }

@@ -11,19 +11,12 @@
 // (surya/layout/model/decoder.py:95-126, surya/table_rec/model/decoder.py:121-155), per-step token logic
 // (surya/layout/__init__.py:111-137, surya/table_rec/__init__.py:62-131).
 #include "../../include/surya_b200.h"
-#include "ops.cuh"
+#include "engine.cuh"
 
 #include <cmath>
-#include <cstring>
 #include <vector>
 
 using namespace sb;
-
-#define CK(call)                 \
-  do {                           \
-    int rc_ = (call);            \
-    if (rc_) return rc_;         \
-  } while (0)
 
 namespace {
 constexpr int GRAPH_GROUP = 8;
@@ -33,8 +26,7 @@ struct sb_layout_engine {
   sb_layout_config c;
   std::vector<const void*> w;
   size_t esz = 2;
-  uint8_t* arena = nullptr;
-  size_t arena_bytes = 0;
+  Arena arena;
   // encoder workspaces
   void *x = nullptr, *h = nullptr, *qkv = nullptr, *ao = nullptr, *mlp = nullptr;
   // decoder state (persistent: the step graphs point at these)
@@ -50,13 +42,9 @@ struct sb_layout_engine {
   float* out_head[4] = {nullptr, nullptr, nullptr, nullptr};
   unsigned char* done = nullptr;
   int Lk = 0;
-  // graphs
-  cudaGraphExec_t g_group = nullptr, g_one = nullptr;
-  const void* graph_key[8] = {nullptr};
-  int graph_batch = 0;
-  long long launches_per_step = 0;
-  cudaStream_t own_stream = nullptr;
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
+  // decode loop: GRAPH_GROUP steps per replay, and one step for the tail
+  StepGraph g_group{"sb_layout_decode", GRAPH_GROUP}, g_one{"sb_layout_decode", 1};
+  EngineStream stream;
 
   int ncol() const { return 6 + c.n_out_heads; }
   // ---- weight table (see include/surya_b200.h)
@@ -76,21 +64,6 @@ struct sb_layout_engine {
   int n_weights() const { return dec_base() + n_tables() + c.dec_layers * SB_LW_DEC_LAYER + SB_LW_DEC_TAIL + (c.kind == 1 ? 5 : 3); }
 };
 
-static size_t al256(size_t v) { return (v + 255) & ~size_t(255); }
-
-static int lin(const sb_layout_engine* e, const void* A, int lda, const void* Wt, int ldw, void* C, int ldc, int M, int N, int K,
-               const void* bias_f32, const void* residual, int ldr, int act, int swiglu, cudaStream_t st, int allow_splitk = 0) {
-  GemmArgs a;
-  a.dtype = e->c.dtype;
-  a.A = A; a.lda = lda; a.W = Wt; a.ldw = ldw; a.C = C; a.ldc = ldc;
-  a.M = M; a.N = N; a.K = K;
-  a.bias = static_cast<const float*>(bias_f32);
-  a.residual = residual; a.ldr = ldr; a.act = act; a.swiglu = swiglu;
-  a.w_constant = 1;
-  a.allow_splitk = allow_splitk;
-  return gemm_launch(a, st);
-}
-
 // ------------------------------------------------------------------------------------------------ Swin encoder
 static int run_encoder(sb_layout_engine* e, const void* pixels, int is_f32, int B, void* out, cudaStream_t st) {
   const sb_layout_config& c = e->c;
@@ -101,7 +74,7 @@ static int run_encoder(sb_layout_engine* e, const void* pixels, int is_f32, int 
   CK(patch_gather(dt, pixels, is_f32, e->h, B, c.in_ch, c.img_h, c.img_w, c.patch, Kp, st));
   long long rows = static_cast<long long>(B) * H * W;
   int C = c.embed_dim;
-  CK(lin(e, e->h, Kp, e->WF(SB_LW_PE_W), Kp, e->x, C, static_cast<int>(rows), C, Kp, e->WF(SB_LW_PE_B), nullptr, 0, ACT_NONE, 0, st));
+  CK(gemm_launch(weight_gemm(dt, e->h, Kp, e->WF(SB_LW_PE_W), Kp, e->x, C, static_cast<int>(rows), C, Kp, e->WF(SB_LW_PE_B)), st));
   CK(layernorm(dt, e->x, e->WF(SB_LW_PE_LN_W), e->WF(SB_LW_PE_LN_B), e->x, static_cast<int>(rows), C, 1e-5f, st));
   void* x = e->x;
   void* alt = e->ao;     // patch merging ping-pongs between the two C-wide buffers
@@ -113,17 +86,17 @@ static int run_encoder(sb_layout_engine* e, const void* pixels, int is_f32, int 
       const int shift = (l % 2 == 1 && (H < W ? H : W) > c.window) ? c.window / 2 : 0;
       void* attn_out = (x == e->x) ? e->ao : e->x;   // any C-wide buffer that is not x
       CK(layernorm(dt, x, e->WL(s, l, SB_LWE_LN1_W), e->WL(s, l, SB_LWE_LN1_B), e->h, R, C, c.enc_ln_eps, st));
-      CK(lin(e, e->h, C, e->WL(s, l, SB_LWE_QKV_W), C, e->qkv, 3 * C, R, 3 * C, C, e->WL(s, l, SB_LWE_QKV_B), nullptr, 0, ACT_NONE,
-             0, st));
+      CK(gemm_launch(weight_gemm(dt, e->h, C, e->WL(s, l, SB_LWE_QKV_W), C, e->qkv, 3 * C, R, 3 * C, C, e->WL(s, l, SB_LWE_QKV_B)), st));
       CK(swin_window_attn(dt, e->qkv, static_cast<const float*>(e->WL(s, l, SB_LWE_QKV_B)), e->WL(s, l, SB_LWE_RPB), attn_out, B, H, W, C, nh,
                           shift, st));
       // x = attn_out @ Wo^T + bo + x   (written over h first, then swapped in: the GEMM must not alias its residual's rows
       // with a different pitch; here both are [R, C] so in-place on x is the same read-then-write per element)
-      CK(lin(e, attn_out, C, e->WL(s, l, SB_LWE_O_W), C, x, C, R, C, C, e->WL(s, l, SB_LWE_O_B), x, C, ACT_NONE, 0, st));
+      CK(gemm_launch(weight_gemm(dt, attn_out, C, e->WL(s, l, SB_LWE_O_W), C, x, C, R, C, C, e->WL(s, l, SB_LWE_O_B), x, C), st));
       CK(layernorm(dt, x, e->WL(s, l, SB_LWE_LN2_W), e->WL(s, l, SB_LWE_LN2_B), e->h, R, C, c.enc_ln_eps, st));
-      CK(lin(e, e->h, C, e->WL(s, l, SB_LWE_FC1_W), C, e->mlp, 4 * C, R, 4 * C, C, e->WL(s, l, SB_LWE_FC1_B), nullptr, 0,
-             ACT_GELU_ERF, 0, st));
-      CK(lin(e, e->mlp, 4 * C, e->WL(s, l, SB_LWE_FC2_W), 4 * C, x, C, R, C, 4 * C, e->WL(s, l, SB_LWE_FC2_B), x, C, ACT_NONE, 0, st));
+      CK(gemm_launch(weight_gemm(dt, e->h, C, e->WL(s, l, SB_LWE_FC1_W), C, e->mlp, 4 * C, R, 4 * C, C, e->WL(s, l, SB_LWE_FC1_B),
+                                 nullptr, 0, ACT_GELU_ERF), st));
+      CK(gemm_launch(weight_gemm(dt, e->mlp, 4 * C, e->WL(s, l, SB_LWE_FC2_W), 4 * C, x, C, R, C, 4 * C, e->WL(s, l, SB_LWE_FC2_B), x,
+                                 C), st));
     }
     if (s < c.n_stages - 1) {
       if ((H | W) & 1) {
@@ -136,7 +109,7 @@ static int run_encoder(sb_layout_engine* e, const void* pixels, int is_f32, int 
       H /= 2; W /= 2;
       CK(layernorm(dt, e->mlp, e->WM(s, 0), e->WM(s, 1), e->mlp, static_cast<int>(rows), 4 * C, 1e-5f, st));
       void* nx = (x == e->x) ? alt : e->x;
-      CK(lin(e, e->mlp, 4 * C, e->WM(s, 2), 4 * C, nx, 2 * C, static_cast<int>(rows), 2 * C, 4 * C, nullptr, nullptr, 0, ACT_NONE, 0, st));
+      CK(gemm_launch(weight_gemm(dt, e->mlp, 4 * C, e->WM(s, 2), 4 * C, nx, 2 * C, static_cast<int>(rows), 2 * C, 4 * C, nullptr), st));
       x = nx;
       C *= 2;
     }
@@ -164,15 +137,15 @@ static int run_token(sb_layout_engine* e, const long long* tok, const int* pos, 
   for (int l = 0; l < c.dec_layers; ++l) {
     // cross attention over the cached encoder K/V
     CK(rmsnorm(dt, e->dx, Hd, e->WD(l, SB_LWD_CROSS_NORM), e->dn, Hd, B, Hd, c.rms_eps, nullptr, st, 1));
-    CK(lin(e, e->dn, Hd, e->WD(l, SB_LWD_CQ_W), Hd, e->dq, nh * hd, B, nh * hd, Hd, nullptr, nullptr, 0, ACT_NONE, 0, st));
+    CK(gemm_launch(weight_gemm(dt, e->dn, Hd, e->WD(l, SB_LWD_CQ_W), Hd, e->dq, nh * hd, B, nh * hd, Hd, nullptr), st));
     const uint8_t* kv = static_cast<const uint8_t*>(e->ckv[l]);
     CK(attn_single_query(dt, e->dq, nh * hd, kv, kv + static_cast<size_t>(nkv) * hd * e->esz, static_cast<long long>(e->Lk) * KVW, hd,
                          KVW, e->da, nh * hd, B, nh, nkv, hd, e->Lk, scale, st));
-    CK(lin(e, e->da, nh * hd, e->WD(l, SB_LWD_CO_W), nh * hd, e->dcross, Hd, B, Hd, nh * hd, e->WD(l, SB_LWD_CO_B), e->dx, Hd, ACT_NONE,
-           0, st));
+    CK(gemm_launch(weight_gemm(dt, e->da, nh * hd, e->WD(l, SB_LWD_CO_W), nh * hd, e->dcross, Hd, B, Hd, nh * hd, e->WD(l, SB_LWD_CO_B),
+                               e->dx, Hd), st));
     // causal self attention (RoPE + cache append fused into the attention kernel)
     CK(rmsnorm(dt, e->dcross, Hd, e->WD(l, SB_LWD_SELF_NORM), e->dn, Hd, B, Hd, c.rms_eps, nullptr, st, 1));
-    CK(lin(e, e->dn, Hd, e->WD(l, SB_LWD_SQKV_W), Hd, e->dqkv, QW, B, QW, Hd, nullptr, nullptr, 0, ACT_NONE, 0, st));
+    CK(gemm_launch(weight_gemm(dt, e->dn, Hd, e->WD(l, SB_LWD_SQKV_W), Hd, e->dqkv, QW, B, QW, Hd, nullptr), st));
     DecodeAttnArgs a;
     a.dtype = dt; a.qkv = e->dqkv; a.ld = QW; a.kcache = e->kc[l]; a.vcache = e->vc[l]; a.slot = e->slot; a.pos = pos;
     a.inv_freq = static_cast<const float*>(e->WX(SB_LWX_INV_FREQ));
@@ -180,12 +153,15 @@ static int run_token(sb_layout_engine* e, const long long* tok, const int* pos, 
     a.scale = scale;
     CK(decode_attn(a, st));
     const void* res_src = c.double_residual ? e->dx : e->dcross;
-    CK(lin(e, e->da, nh * hd, e->WD(l, SB_LWD_SO_W), nh * hd, e->dres, Hd, B, Hd, nh * hd, e->WD(l, SB_LWD_SO_B), res_src, Hd, ACT_NONE,
-           0, st));
+    CK(gemm_launch(weight_gemm(dt, e->da, nh * hd, e->WD(l, SB_LWD_SO_W), nh * hd, e->dres, Hd, B, Hd, nh * hd, e->WD(l, SB_LWD_SO_B),
+                               res_src, Hd), st));
     // GeGLU MLP
     CK(rmsnorm(dt, e->dres, Hd, e->WD(l, SB_LWD_MLP_NORM), e->dn, Hd, B, Hd, c.rms_eps, nullptr, st, 1));
-    CK(lin(e, e->dn, Hd, e->WD(l, SB_LWD_GU_W), Hd, e->dm, c.inter, B, 2 * c.inter, Hd, nullptr, nullptr, 0, ACT_GELU_TANH, 1, st));
-    CK(lin(e, e->dm, c.inter, e->WD(l, SB_LWD_DOWN_W), c.inter, e->dx, Hd, B, Hd, c.inter, nullptr, e->dres, Hd, ACT_NONE, 0, st, 1));
+    CK(gemm_launch(weight_gemm(dt, e->dn, Hd, e->WD(l, SB_LWD_GU_W), Hd, e->dm, c.inter, B, 2 * c.inter, Hd, nullptr, nullptr, 0,
+                               ACT_GELU_TANH, 1), st));
+    GemmArgs down = weight_gemm(dt, e->dm, c.inter, e->WD(l, SB_LWD_DOWN_W), c.inter, e->dx, Hd, B, Hd, c.inter, nullptr, e->dres, Hd);
+    down.allow_splitk = 1;
+    CK(gemm_launch(down, st));
   }
   CK(rmsnorm(dt, e->dx, Hd, e->WX(SB_LWX_FINAL_NORM), e->dn, Hd, B, Hd, c.rms_eps, nullptr, st, 1));
   CK(layernorm(dt, e->dn, e->WX(SB_LWX_OUT_LN_W), e->WX(SB_LWX_OUT_LN_B), e->dh, B, Hd, c.dec_ln_eps, st));
@@ -250,36 +226,24 @@ int sb_layout_create(const sb_layout_config* cfg, const void* const* weights, in
   const size_t Lk = static_cast<size_t>(Hl) * Wl;
   const size_t Hd = c.hidden, QW = (c.n_heads + 2 * c.n_kv) * c.head_dim, KVW = 2 * c.n_kv * c.head_dim;
   const size_t cache = B * c.n_kv * c.s_max * c.head_dim * es;
-  std::vector<size_t> sizes = {
-      rows0 * C0 * es, rows0 * hcols * es, rows0 * 3 * C0 * es, rows0 * C0 * es, rows0 * 4 * C0 * es,           // x h qkv ao mlp
-      B * Hd * es, B * Hd * es, B * c.n_heads * c.head_dim * es, B * c.n_heads * c.head_dim * es, B * Hd * es,  // dx dn dq da dcross
-      B * Hd * es, B * QW * es, B * c.inter * es, B * Hd * es,                                                  // dres dqkv dm dh
-      B * Lk * c.enc_hidden * es,                                                                               // enc
-      B * sizeof(int), B * 10 * sizeof(long long), B * sizeof(int), 256, B * 6 * sizeof(float), B,              // slot tok pos base bbox done
-  };
-  for (int k = 0; k < 4; ++k) sizes.push_back(B * (k < c.n_out_heads ? c.head_n[k] : 1) * sizeof(float));
-  for (int l = 0; l < c.dec_layers; ++l) { sizes.push_back(B * Lk * KVW * es); sizes.push_back(cache); sizes.push_back(cache); }
-  size_t total = 0;
-  for (size_t s : sizes) total += al256(s);
-  if (cudaMalloc(&e->arena, total) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("sb_layout_create: cudaMalloc(%zu) failed", total);
+  const size_t QH = static_cast<size_t>(c.n_heads) * c.head_dim;
+  Arena& a = e->arena;
+  a.add(e->x, rows0 * C0 * es); a.add(e->h, rows0 * hcols * es); a.add(e->qkv, rows0 * 3 * C0 * es); a.add(e->ao, rows0 * C0 * es);
+  a.add(e->mlp, rows0 * 4 * C0 * es);
+  a.add(e->dx, B * Hd * es); a.add(e->dn, B * Hd * es); a.add(e->dq, B * QH * es); a.add(e->da, B * QH * es);
+  a.add(e->dcross, B * Hd * es); a.add(e->dres, B * Hd * es); a.add(e->dqkv, B * QW * es); a.add(e->dm, B * c.inter * es);
+  a.add(e->dh, B * Hd * es);
+  a.add(e->enc, B * Lk * c.enc_hidden * es);
+  a.add(e->slot, B * sizeof(int)); a.add(e->tok, B * 10 * sizeof(long long)); a.add(e->pos, B * sizeof(int)); a.add(e->base, 256);
+  a.add(e->out_bbox, B * 6 * sizeof(float)); a.add(e->done, B);
+  for (int k = 0; k < 4; ++k) a.add(e->out_head[k], B * (k < c.n_out_heads ? c.head_n[k] : 1) * sizeof(float));
+  e->ckv.resize(c.dec_layers); e->kc.resize(c.dec_layers); e->vc.resize(c.dec_layers);
+  for (int l = 0; l < c.dec_layers; ++l) { a.add(e->ckv[l], B * Lk * KVW * es); a.add(e->kc[l], cache); a.add(e->vc[l], cache); }
+  if (a.alloc() != cudaSuccess) {
+    set_error("sb_layout_create: cudaMalloc(%zu) failed", a.bytes());
     delete e;
     return -5;
   }
-  cudaMemset(e->arena, 0, total);
-  e->arena_bytes = total;
-  uint8_t* p = e->arena;
-  size_t si = 0;
-  auto take = [&]() { void* r = p; p += al256(sizes[si++]); return r; };
-  e->x = take(); e->h = take(); e->qkv = take(); e->ao = take(); e->mlp = take();
-  e->dx = take(); e->dn = take(); e->dq = take(); e->da = take(); e->dcross = take();
-  e->dres = take(); e->dqkv = take(); e->dm = take(); e->dh = take();
-  e->enc = take();
-  e->slot = static_cast<int*>(take()); e->tok = static_cast<long long*>(take()); e->pos = static_cast<int*>(take());
-  e->base = static_cast<int*>(take()); e->out_bbox = static_cast<float*>(take()); e->done = static_cast<unsigned char*>(take());
-  for (int k = 0; k < 4; ++k) e->out_head[k] = static_cast<float*>(take());
-  for (int l = 0; l < c.dec_layers; ++l) { e->ckv.push_back(take()); e->kc.push_back(take()); e->vc.push_back(take()); }
   std::vector<int> slots(B);
   for (size_t i = 0; i < B; ++i) slots[i] = static_cast<int>(i);
   cudaMemcpy(e->slot, slots.data(), B * sizeof(int), cudaMemcpyHostToDevice);
@@ -288,18 +252,9 @@ int sb_layout_create(const sb_layout_config* cfg, const void* const* weights, in
   return 0;
 }
 
-void sb_layout_destroy(sb_layout_engine* e) {
-  if (!e) return;
-  if (e->g_group) cudaGraphExecDestroy(e->g_group);
-  if (e->g_one) cudaGraphExecDestroy(e->g_one);
-  if (e->ev_in) cudaEventDestroy(e->ev_in);
-  if (e->ev_out) cudaEventDestroy(e->ev_out);
-  if (e->own_stream) cudaStreamDestroy(e->own_stream);
-  if (e->arena) cudaFree(e->arena);
-  delete e;
-}
+void sb_layout_destroy(sb_layout_engine* e) { delete e; }
 
-size_t sb_layout_workspace_bytes(const sb_layout_engine* e) { return e ? e->arena_bytes : 0; }
+size_t sb_layout_workspace_bytes(const sb_layout_engine* e) { return e ? e->arena.bytes() : 0; }
 
 int sb_layout_encode(sb_layout_engine* e, const void* pixels, int pixels_f32, int batch, void* enc_out, void* stream) {
   if (!e || !pixels || !enc_out) { set_error("sb_layout_encode: null argument"); return -1; }
@@ -314,27 +269,9 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
   const sb_layout_config& c = e->c;
   if (batch <= 0 || batch > c.max_batch) { set_error("sb_layout_decode: batch %d outside 1..%d", batch, c.max_batch); return -2; }
   if (q_len < 1 || n_steps < 1 || q_len - 1 + n_steps > c.s_max) { set_error("sb_layout_decode: prompt + steps exceed s_max %d", c.s_max); return -3; }
-  cudaStream_t caller = static_cast<cudaStream_t>(stream);
-  cudaStream_t st = caller;
-  const bool hop = use_graph && (caller == nullptr || caller == cudaStreamLegacy || caller == cudaStreamPerThread);
-  if (hop) {
-    if (!e->own_stream) {
-      if (cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-          cudaEventCreateWithFlags(&e->ev_in, cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreateWithFlags(&e->ev_out, cudaEventDisableTiming) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("sb_layout_decode: could not create the engine stream");
-        return -8;
-      }
-    }
-    cudaEventRecord(e->ev_in, caller);
-    cudaStreamWaitEvent(e->own_stream, e->ev_in, 0);
-    st = e->own_stream;
-  }
-  struct Rejoin {
-    bool on; cudaStream_t own, caller; cudaEvent_t ev;
-    ~Rejoin() { if (on) { cudaEventRecord(ev, own); cudaStreamWaitEvent(caller, ev, 0); } }
-  } rejoin{hop, e->own_stream, caller, e->ev_out};
+  Hop hop(e->stream, static_cast<cudaStream_t>(stream), use_graph);
+  if (hop.failed) { set_error("sb_layout_decode: could not create the engine stream"); return -8; }
+  const cudaStream_t st = hop.st;
 
   const int B = batch, ncol = e->ncol();
   const size_t es = e->esz;
@@ -345,8 +282,8 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
   }
   const int KVW = 2 * c.n_kv * c.head_dim;
   for (int l = 0; l < c.dec_layers; ++l)
-    CK(lin(e, e->enc, c.enc_hidden, e->WD(l, SB_LWD_CKV_W), c.enc_hidden, e->ckv[l], KVW, B * e->Lk, KVW, c.enc_hidden, nullptr, nullptr, 0,
-           ACT_NONE, 0, st));
+    CK(gemm_launch(weight_gemm(c.dtype, e->enc, c.enc_hidden, e->WD(l, SB_LWD_CKV_W), c.enc_hidden, e->ckv[l], KVW, B * e->Lk, KVW,
+                               c.enc_hidden, nullptr), st));
   // prompt: all but the last token, position by position (identical to the batched prefill under the causal mask)
   std::vector<int> hpos(B);
   for (int j = 0; j < q_len; ++j) {
@@ -380,42 +317,14 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
     for (int i = 0; i < left; ++i) CK(body(st));
     return 0;
   }
-  const void* key[8] = {hist_tok, hist_bbox, hist_done, hist_heads ? hist_heads[0] : nullptr,
-                        reinterpret_cast<const void*>(static_cast<uintptr_t>(n_steps)), nullptr, nullptr, nullptr};
-  const bool hit = e->g_one && e->graph_batch == B && std::memcmp(key, e->graph_key, sizeof(key)) == 0;
-  if (!hit) {
-    if (e->g_group) { cudaGraphExecDestroy(e->g_group); e->g_group = nullptr; }
-    if (e->g_one) { cudaGraphExecDestroy(e->g_one); e->g_one = nullptr; }
-    for (int which = 0; which < 2; ++which) {
-      const int k = which == 0 ? GRAPH_GROUP : 1;
-      cudaGraph_t graph = nullptr;
-      cudaError_t cb = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-      if (cb != cudaSuccess) { cudaGetLastError(); set_error("sb_layout_decode: capture begin failed: %s", cudaGetErrorString(cb)); return -6; }
-      const long long before = launch_count();
-      int rc = 0;
-      for (int i = 0; i < k && !rc; ++i) rc = body(st);
-      e->launches_per_step = (launch_count() - before) / k;
-      count_launches(before - launch_count());   // captured, not executed
-      cudaError_t ce = cudaStreamEndCapture(st, &graph);
-      if (rc || ce != cudaSuccess) { cudaGetLastError(); set_error("sb_layout_decode: capture failed: rc=%d %s", rc, cudaGetErrorString(ce)); return -6; }
-      ce = cudaGraphInstantiate(which == 0 ? &e->g_group : &e->g_one, graph, 0);
-      cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) { cudaGetLastError(); set_error("sb_layout_decode: instantiate failed: %s", cudaGetErrorString(ce)); return -7; }
-    }
-    e->graph_batch = B;
-    std::memcpy(e->graph_key, key, sizeof(key));
+  const StepGraph::Key key = {hist_tok, hist_bbox, hist_done, hist_heads ? hist_heads[0] : nullptr,
+                              reinterpret_cast<const void*>(static_cast<uintptr_t>(n_steps))};
+  if (!e->g_group.hit(key, B) || !e->g_one.hit(key, B)) {
+    CK(e->g_group.capture(key, B, st, body));
+    CK(e->g_one.capture(key, B, st, body));
   }
-  const long long per_step = e->launches_per_step;   // kernels per step as counted while capturing (launch accounting)
-  while (left >= GRAPH_GROUP) {
-    if (cudaGraphLaunch(e->g_group, st) != cudaSuccess) { cudaGetLastError(); set_error("sb_layout_decode: graph launch failed"); return -9; }
-    count_launches(per_step * GRAPH_GROUP);
-    left -= GRAPH_GROUP;
-  }
-  for (; left > 0; --left) {
-    if (cudaGraphLaunch(e->g_one, st) != cudaSuccess) { cudaGetLastError(); set_error("sb_layout_decode: graph launch failed"); return -9; }
-    count_launches(per_step);
-  }
-  return 0;
+  CK(e->g_group.replay(left / GRAPH_GROUP, st));
+  return e->g_one.replay(left % GRAPH_GROUP, st);
 }
 
 }  // extern "C"

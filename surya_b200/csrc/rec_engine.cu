@@ -5,28 +5,20 @@
 // decode step is 62 back-to-back kernel launches on one stream (5 per decoder layer + lm_head + tail), capturable into a
 // CUDA graph and replayed with token feedback / position increment / history done on the device (sb_rec_decode_steps).
 #include "../../include/surya_b200.h"
-#include "ops.cuh"
+#include "engine.cuh"
 #include "sb_ptx.cuh"
 
-#include <cstring>
 #include <string>
 #include <vector>
 
 using namespace sb;
-
-#define CK(x)                    \
-  do {                           \
-    int rc_ = (x);               \
-    if (rc_) return rc_;         \
-  } while (0)
 
 struct sb_rec_engine {
   sb_rec_config c;
   std::vector<const void*> w;
   size_t esz = 2;
   // workspaces (device)
-  uint8_t* arena = nullptr;
-  size_t arena_bytes = 0;
+  Arena arena;
   void *x = nullptr, *nbuf = nullptr, *qkv = nullptr, *ao = nullptr, *act = nullptr, *x0 = nullptr, *m1 = nullptr,
        *feat = nullptr, *xl = nullptr, *logits = nullptr;
   void* kcache = nullptr;  // [layer][slot][kvh][s_max][d]
@@ -40,14 +32,9 @@ struct sb_rec_engine {
   float* am_val = nullptr; int* am_idx = nullptr; float* am_sum = nullptr;
   int am_ld = 0, am_bn = 0;
   int qkv_w_enc = 0, qkv_w_dec = 0;
-  // CUDA graph cache for decode_steps
-  cudaGraphExec_t graph_exec = nullptr;
-  int graph_batch = 0;
-  long long graph_nodes = 0;
-  // the legacy default stream cannot be captured: decode_steps hops onto an engine-owned stream, ordered by events
-  cudaStream_t own_stream = nullptr;
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-  const void* graph_key[8] = {nullptr};
+  // decode_steps: one captured step, replayed
+  StepGraph graph{"sb_rec_decode_steps", 1};
+  EngineStream stream;
   // device-side stop rules (sb_rec_set_sched): caller-owned per-row state, evaluated by stop_rules_kernel after every loop step
   int* sc_gen = nullptr; long long* sc_ring = nullptr; unsigned char* sc_done = nullptr; int* sc_valid = nullptr; int* sc_active = nullptr;
   int sc_max_tokens = 0, sc_max_repeats = 0;
@@ -65,27 +52,6 @@ struct sb_rec_engine {
   }
 };
 
-static size_t al256(size_t v) { return (v + 255) & ~size_t(255); }
-
-// norm: 0 = plain, 1 = folded RMSNorm with the per-row scale in e->rs (prefill), 2 = folded RMSNorm with the scale computed
-// inside the GEMM from the A tiles (decode steps, lm_head)
-static int linear(const sb_rec_engine* e, const void* A, int lda, const void* Wt, int ldw, void* C, int ldc, int M, int N,
-                  int K, const void* bias_f32, const void* residual, int ldr, int act, int swiglu, cudaStream_t st,
-                  int allow_splitk = 0, int norm = 0, int decode = 0) {
-  GemmArgs a;
-  if (norm == 1) a.rowscale = e->rs;
-  if (norm == 2) { a.ssq_inline = 1; a.ssq_eps = e->c.rms_eps; a.ssq_k = K; }
-  a.dtype = e->c.dtype;
-  a.A = A; a.lda = lda; a.W = Wt; a.ldw = ldw; a.C = C; a.ldc = ldc;
-  a.M = M; a.N = N; a.K = K;
-  a.bias = static_cast<const float*>(bias_f32);
-  a.residual = residual; a.ldr = ldr; a.act = act; a.swiglu = swiglu;
-  a.w_constant = 1;   // engine weights are never written after packing
-  a.allow_splitk = allow_splitk;
-  a.decode = decode;
-  return gemm_launch(a, st);
-}
-
 // ------------------------------------------------------------------------------------------------ vision tower
 static int run_vision(sb_rec_engine* e, const void* tiles, int tiles_f32, int n, const int* perm, const int* pos_rc,
                       const int* win_start, const int* win_len, int n_win, int max_win, const int* img_start,
@@ -94,14 +60,13 @@ static int run_vision(sb_rec_engine* e, const void* tiles, int tiles_f32, int n,
   const int H = c.enc_hidden, nh = c.enc_heads, hd = H / nh;
   const int dt = c.dtype;
   CK(gather_pad_rows(dt, tiles, tiles_f32, c.patch_dim, perm, e->x0, c.patch_dim_pad, n, c.patch_dim, c.patch_dim_pad, st));
-  CK(linear(e, e->x0, c.patch_dim_pad, e->W(SB_RW_PATCH_W), c.patch_dim_pad, e->x, H, n, H, c.patch_dim_pad, nullptr,
-            nullptr, 0, ACT_NONE, 0, st));
+  CK(gemm_launch(weight_gemm(dt, e->x0, c.patch_dim_pad, e->W(SB_RW_PATCH_W), c.patch_dim_pad, e->x, H, n, H, c.patch_dim_pad,
+                             nullptr), st));
   const int ldq = 3 * H;
   uint8_t* qkv8 = static_cast<uint8_t*>(e->qkv);
   for (int l = 0; l < c.enc_depth; ++l) {
     CK(rmsnorm(dt, e->x, H, e->WE(l, SB_RWE_NORM1), e->nbuf, H, n, H, 1e-6f, nullptr, st));
-    CK(linear(e, e->nbuf, H, e->WE(l, SB_RWE_QKV_W), H, e->qkv, ldq, n, 3 * H, H, e->WE(l, SB_RWE_QKV_B), nullptr, 0,
-              ACT_NONE, 0, st));
+    CK(gemm_launch(weight_gemm(dt, e->nbuf, H, e->WE(l, SB_RWE_QKV_W), H, e->qkv, ldq, n, 3 * H, H, e->WE(l, SB_RWE_QKV_B)), st));
     CK(rope_vision(dt, e->qkv, ldq, pos_rc, static_cast<const float*>(e->W(SB_RW_ENC_INV_FREQ)), n, nh, hd, st));
     AttnArgs a;
     a.dtype = dt;
@@ -117,20 +82,20 @@ static int run_vision(sb_rec_engine* e, const void* tiles, int tiles_f32, int n,
     a.n_heads = nh; a.n_kv_heads = nh; a.head_dim = hd; a.causal = 0;
     a.scale = 1.0f / sqrtf(static_cast<float>(hd));
     CK(attn_varlen(a, st));
-    CK(linear(e, e->ao, H, e->WE(l, SB_RWE_PROJ_W), H, e->x, H, n, H, H, e->WE(l, SB_RWE_PROJ_B), e->x, H, ACT_NONE, 0, st));
+    CK(gemm_launch(weight_gemm(dt, e->ao, H, e->WE(l, SB_RWE_PROJ_W), H, e->x, H, n, H, H, e->WE(l, SB_RWE_PROJ_B), e->x, H), st));
     CK(rmsnorm(dt, e->x, H, e->WE(l, SB_RWE_NORM2), e->nbuf, H, n, H, 1e-6f, nullptr, st));
-    CK(linear(e, e->nbuf, H, e->WE(l, SB_RWE_GU_W), H, e->act, c.enc_inter_pad, n, 2 * c.enc_inter_pad, H,
-              e->WE(l, SB_RWE_GU_B), nullptr, 0, ACT_SILU, 1, st));
-    CK(linear(e, e->act, c.enc_inter_pad, e->WE(l, SB_RWE_DOWN_W), c.enc_inter_pad, e->x, H, n, H, c.enc_inter_pad,
-              e->WE(l, SB_RWE_DOWN_B), e->x, H, ACT_NONE, 0, st));
+    CK(gemm_launch(weight_gemm(dt, e->nbuf, H, e->WE(l, SB_RWE_GU_W), H, e->act, c.enc_inter_pad, n, 2 * c.enc_inter_pad, H,
+                               e->WE(l, SB_RWE_GU_B), nullptr, 0, ACT_SILU, 1), st));
+    CK(gemm_launch(weight_gemm(dt, e->act, c.enc_inter_pad, e->WE(l, SB_RWE_DOWN_W), c.enc_inter_pad, e->x, H, n, H,
+                               c.enc_inter_pad, e->WE(l, SB_RWE_DOWN_B), e->x, H), st));
   }
   // merger: RMSNorm -> view [n/unit, unit*H] -> Linear+GELU -> Linear
   const int mu = c.merge_unit, MH = mu * H, nm = n / mu;
   CK(rmsnorm(dt, e->x, H, e->W(SB_RW_MERGER_LN), e->nbuf, H, n, H, 1e-6f, nullptr, st));
-  CK(linear(e, e->nbuf, MH, e->W(SB_RW_MERGER_W0), MH, e->m1, MH, nm, MH, MH, e->W(SB_RW_MERGER_B0), nullptr, 0,
-            ACT_GELU_ERF, 0, st));
-  CK(linear(e, e->m1, MH, e->W(SB_RW_MERGER_W2), MH, e->feat, c.enc_out_hidden, nm, c.enc_out_hidden, MH,
-            e->W(SB_RW_MERGER_B2), nullptr, 0, ACT_NONE, 0, st));
+  CK(gemm_launch(weight_gemm(dt, e->nbuf, MH, e->W(SB_RW_MERGER_W0), MH, e->m1, MH, nm, MH, MH, e->W(SB_RW_MERGER_B0), nullptr, 0,
+                             ACT_GELU_ERF), st));
+  CK(gemm_launch(weight_gemm(dt, e->m1, MH, e->W(SB_RW_MERGER_W2), MH, e->feat, c.enc_out_hidden, nm, c.enc_out_hidden, MH,
+                             e->W(SB_RW_MERGER_B2)), st));
   return 0;
 }
 
@@ -152,13 +117,8 @@ struct HeadOut {
 static int run_heads(sb_rec_engine* e, void* hidden, int rows, const HeadOut& o, cudaStream_t st) {
   const sb_rec_config& c = e->c;
   const int D = c.dec_hidden;
-  GemmArgs a;
-  a.dtype = c.dtype;
-  a.A = hidden; a.lda = D; a.W = e->W(SB_RW_LM_W); a.ldw = D;
-  a.C = o.logits ? o.logits : e->logits; a.ldc = c.vocab;
-  a.M = rows; a.N = c.vocab; a.K = D;
-  a.bias = static_cast<const float*>(e->W(SB_RW_LM_BIAS));
-  a.w_constant = 1;
+  GemmArgs a = weight_gemm(c.dtype, hidden, D, e->W(SB_RW_LM_W), D, o.logits ? o.logits : e->logits, c.vocab, rows, c.vocab, D,
+                           e->W(SB_RW_LM_BIAS));
   // 1/rms of the final norm: separate pass + rowscale rather than the in-kernel sum of squares — this GEMM has hundreds of
   // column tiles per row block, and the in-kernel pass would recompute the rows' sum of squares for every one of them
   CK(row_rstd(c.dtype, hidden, D, e->rs, rows, D, c.rms_eps, nullptr, st));
@@ -204,8 +164,9 @@ static int run_decoder_prefill(sb_rec_engine* e, const long long* ids, int n_tok
   uint8_t* qkv8 = static_cast<uint8_t*>(e->qkv);
   for (int l = 0; l < c.dec_layers; ++l) {
     CK(row_rstd(dt, e->x, D, e->rs, n_tok, D, c.rms_eps, nullptr, st));
-    CK(linear(e, e->x, D, e->WD(l, SB_RWD_QKV_W), D, e->qkv, Q, n_tok, Q, D, e->WD(l, SB_RWD_QKV_B), nullptr, 0, ACT_NONE, 0,
-              st, 0, /*norm=*/1));
+    GemmArgs qkv = weight_gemm(dt, e->x, D, e->WD(l, SB_RWD_QKV_W), D, e->qkv, Q, n_tok, Q, D, e->WD(l, SB_RWD_QKV_B));
+    qkv.rowscale = e->rs;
+    CK(gemm_launch(qkv, st));
     CK(rope_kv_append(dt, e->qkv, Q, tok_pos, tok_slot, static_cast<const float*>(e->W(SB_RW_DEC_INV_FREQ)), e->kc(l),
                       e->vc(l), n_tok, nh, nkv, hd, c.s_max, st));
     AttnArgs a;
@@ -218,12 +179,14 @@ static int run_decoder_prefill(sb_rec_engine* e, const long long* ids, int n_tok
     a.n_heads = nh; a.n_kv_heads = nkv; a.head_dim = hd; a.causal = 1;
     a.scale = 1.0f / sqrtf(static_cast<float>(hd));
     CK(attn_varlen(a, st));
-    CK(linear(e, e->ao, nh * hd, e->WD(l, SB_RWD_O_W), nh * hd, e->x, D, n_tok, D, nh * hd, nullptr, e->x, D, ACT_NONE, 0, st));
+    CK(gemm_launch(weight_gemm(dt, e->ao, nh * hd, e->WD(l, SB_RWD_O_W), nh * hd, e->x, D, n_tok, D, nh * hd, nullptr, e->x, D), st));
     CK(row_rstd(dt, e->x, D, e->rs, n_tok, D, c.rms_eps, nullptr, st));
-    CK(linear(e, e->x, D, e->WD(l, SB_RWD_GU_W), D, e->act, c.dec_inter_pad, n_tok, 2 * c.dec_inter_pad, D, nullptr, nullptr, 0,
-              ACT_SILU, 1, st, 0, /*norm=*/1));
-    CK(linear(e, e->act, c.dec_inter_pad, e->WD(l, SB_RWD_DOWN_W), c.dec_inter_pad, e->x, D, n_tok, D, c.dec_inter_pad,
-              nullptr, e->x, D, ACT_NONE, 0, st));
+    GemmArgs gu = weight_gemm(dt, e->x, D, e->WD(l, SB_RWD_GU_W), D, e->act, c.dec_inter_pad, n_tok, 2 * c.dec_inter_pad, D,
+                              nullptr, nullptr, 0, ACT_SILU, 1);
+    gu.rowscale = e->rs;
+    CK(gemm_launch(gu, st));
+    CK(gemm_launch(weight_gemm(dt, e->act, c.dec_inter_pad, e->WD(l, SB_RWD_DOWN_W), c.dec_inter_pad, e->x, D, n_tok, D,
+                               c.dec_inter_pad, nullptr, e->x, D), st));
   }
   // hidden[:, -1:, :] (surya/common/surya/__init__.py:323): the last real token of every sequence, still un-normalised
   CK(gather_pad_rows(dt, e->x, 0, D, last_tok, e->xl, D, n_seq, D, D, st));
@@ -243,19 +206,26 @@ static int run_decode_step(sb_rec_engine* e, const long long* ids, const int* sl
   const int dec = B <= 256 ? 1 : 0;
   if (ids) CK(embed_rows(dt, ids, e->W(SB_RW_EMBED), x, D, B, D, st));
   for (int l = 0; l < c.dec_layers; ++l) {
-    CK(linear(e, x, D, e->WD(l, SB_RWD_QKV_W), D, e->qkv, Q, B, Q, D, e->WD(l, SB_RWD_QKV_B), nullptr, 0, ACT_NONE, 0, st, 0,
-              /*norm=*/2, dec));
+    GemmArgs qkv = weight_gemm(dt, x, D, e->WD(l, SB_RWD_QKV_W), D, e->qkv, Q, B, Q, D, e->WD(l, SB_RWD_QKV_B));
+    qkv.ssq_inline = 1; qkv.ssq_eps = c.rms_eps; qkv.ssq_k = D; qkv.decode = dec;
+    CK(gemm_launch(qkv, st));
     DecodeAttnArgs a;
     a.dtype = dt; a.qkv = e->qkv; a.ld = Q; a.kcache = e->kc(l); a.vcache = e->vc(l); a.slot = slot; a.pos = pos;
     a.inv_freq = static_cast<const float*>(e->W(SB_RW_DEC_INV_FREQ));
     a.out = e->ao; a.ldo = nh * hd; a.batch = B; a.n_heads = nh; a.n_kv_heads = nkv; a.head_dim = hd; a.s_max = c.s_max;
     a.scale = 1.0f / sqrtf(static_cast<float>(hd));
     CK(decode_attn(a, st));
-    CK(linear(e, e->ao, nh * hd, e->WD(l, SB_RWD_O_W), nh * hd, x, D, B, D, nh * hd, nullptr, x, D, ACT_NONE, 0, st, 0, 0, dec));
-    CK(linear(e, x, D, e->WD(l, SB_RWD_GU_W), D, e->act, c.dec_inter_pad, B, 2 * c.dec_inter_pad, D, nullptr, nullptr, 0,
-              ACT_SILU, 1, st, 0, /*norm=*/2, dec));
-    CK(linear(e, e->act, c.dec_inter_pad, e->WD(l, SB_RWD_DOWN_W), c.dec_inter_pad, x, D, B, D, c.dec_inter_pad, nullptr, x, D,
-              ACT_NONE, 0, st, /*allow_splitk=*/1));
+    GemmArgs o = weight_gemm(dt, e->ao, nh * hd, e->WD(l, SB_RWD_O_W), nh * hd, x, D, B, D, nh * hd, nullptr, x, D);
+    o.decode = dec;
+    CK(gemm_launch(o, st));
+    GemmArgs gu = weight_gemm(dt, x, D, e->WD(l, SB_RWD_GU_W), D, e->act, c.dec_inter_pad, B, 2 * c.dec_inter_pad, D, nullptr,
+                              nullptr, 0, ACT_SILU, 1);
+    gu.ssq_inline = 1; gu.ssq_eps = c.rms_eps; gu.ssq_k = D; gu.decode = dec;
+    CK(gemm_launch(gu, st));
+    GemmArgs down = weight_gemm(dt, e->act, c.dec_inter_pad, e->WD(l, SB_RWD_DOWN_W), c.dec_inter_pad, x, D, B, D, c.dec_inter_pad,
+                                nullptr, x, D);
+    down.allow_splitk = 1;
+    CK(gemm_launch(down, st));
   }
   return run_heads(e, x, B, out, st);
 }
@@ -291,47 +261,28 @@ int sb_rec_create(const sb_rec_config* cfg, const void* const* weights, int n_we
   e->am_bn = gemm_argmax_tile(static_cast<int>(rows_out), c.vocab);
   e->am_ld = (c.vocab + e->am_bn - 1) / e->am_bn;
   const size_t am_elems = rows_out * static_cast<size_t>(e->am_ld);
-  size_t sizes[] = {
-      R * Hm * es, R * Hm * es, R * qkvw * es, R * aow * es, R * actw * es,           // x nbuf qkv ao act
-      (size_t)c.max_patches * c.patch_dim_pad * es, nm * c.merge_unit * c.enc_hidden * es,  // x0 m1
-      nm * c.enc_out_hidden * es, rows_out * c.dec_hidden * es, rows_out * c.vocab * es,   // feat xl logits
-      kv_bytes, kv_bytes,
-      rows_out * 8, rows_out * 4, rows_out * 6 * 8, rows_out, rows_out * 8, 256, 256,
-      R * 4, am_elems * 4, am_elems * 4, am_elems * 4};
-  size_t total = 0;
-  for (size_t s : sizes) total += al256(s);
-  cudaError_t ce = cudaMalloc(&e->arena, total);
+  Arena& a = e->arena;
+  a.add(e->x, R * Hm * es); a.add(e->nbuf, R * Hm * es); a.add(e->qkv, R * qkvw * es); a.add(e->ao, R * aow * es);
+  a.add(e->act, R * actw * es);
+  a.add(e->x0, (size_t)c.max_patches * c.patch_dim_pad * es); a.add(e->m1, nm * c.merge_unit * c.enc_hidden * es);
+  a.add(e->feat, nm * c.enc_out_hidden * es); a.add(e->xl, rows_out * c.dec_hidden * es); a.add(e->logits, rows_out * c.vocab * es);
+  a.add(e->kcache, kv_bytes); a.add(e->vcache, kv_bytes);
+  a.add(e->st_tok, rows_out * 8); a.add(e->st_score, rows_out * 4); a.add(e->st_bbox, rows_out * 6 * 8); a.add(e->st_done, rows_out);
+  a.add(e->st_next, rows_out * 8); a.add(e->st_step, 256); a.add(e->st_counter, 256);
+  a.add(e->rs, R * 4); a.add(e->am_val, am_elems * 4); a.add(e->am_idx, am_elems * 4); a.add(e->am_sum, am_elems * 4);
+  cudaError_t ce = a.alloc();
   if (ce != cudaSuccess) {
-    set_error("sb_rec_create: cudaMalloc(%zu MiB) failed: %s", total >> 20, cudaGetErrorString(ce));
+    set_error("sb_rec_create: cudaMalloc(%zu MiB) failed: %s", a.bytes() >> 20, cudaGetErrorString(ce));
     delete e;
     return -6;
   }
-  e->arena_bytes = total;
-  uint8_t* p = e->arena;
-  void** slots[] = {&e->x, &e->nbuf, &e->qkv, &e->ao, &e->act, &e->x0, &e->m1, &e->feat, &e->xl, &e->logits,
-                    &e->kcache, &e->vcache, (void**)&e->st_tok, (void**)&e->st_score, (void**)&e->st_bbox,
-                    (void**)&e->st_done, (void**)&e->st_next, (void**)&e->st_step, (void**)&e->st_counter,
-                    (void**)&e->rs, (void**)&e->am_val, (void**)&e->am_idx, (void**)&e->am_sum};
-  for (size_t i = 0; i < sizeof(sizes) / sizeof(sizes[0]); ++i) {
-    *slots[i] = p;
-    p += al256(sizes[i]);
-  }
-  cudaMemset(e->arena, 0, total);
   *out = e;
   return 0;
 }
 
-void sb_rec_destroy(sb_rec_engine* e) {
-  if (!e) return;
-  if (e->graph_exec) cudaGraphExecDestroy(e->graph_exec);
-  if (e->ev_in) cudaEventDestroy(e->ev_in);
-  if (e->ev_out) cudaEventDestroy(e->ev_out);
-  if (e->own_stream) cudaStreamDestroy(e->own_stream);
-  if (e->arena) cudaFree(e->arena);
-  delete e;
-}
+void sb_rec_destroy(sb_rec_engine* e) { delete e; }
 
-size_t sb_rec_workspace_bytes(const sb_rec_engine* e) { return e ? e->arena_bytes : 0; }
+size_t sb_rec_workspace_bytes(const sb_rec_engine* e) { return e ? e->arena.bytes() : 0; }
 
 int sb_rec_prefill(sb_rec_engine* e, const void* tiles, int tiles_f32, int n_patches, const int* patch_perm,
                    const int* patch_pos_rc, const int* win_start, const int* win_len, int n_win, int max_win_len,
@@ -375,27 +326,9 @@ int sb_rec_decode_steps(sb_rec_engine* e, long long* ids_io, const int* slot, in
                         int use_graph, void* stream) {
   if (!e) { set_error("sb_rec_decode_steps: null engine"); return -1; }
   if (batch > e->c.max_slots || batch > e->c.max_tokens) { set_error("sb_rec_decode_steps: batch exceeds capacity"); return -2; }
-  cudaStream_t caller = static_cast<cudaStream_t>(stream);
-  cudaStream_t st = caller;
-  const bool hop = use_graph && (caller == nullptr || caller == cudaStreamLegacy || caller == cudaStreamPerThread);
-  if (hop) {
-    if (!e->own_stream) {
-      if (cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-          cudaEventCreateWithFlags(&e->ev_in, cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreateWithFlags(&e->ev_out, cudaEventDisableTiming) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("sb_rec_decode_steps: could not create the engine stream");
-        return -8;
-      }
-    }
-    cudaEventRecord(e->ev_in, caller);
-    cudaStreamWaitEvent(e->own_stream, e->ev_in, 0);
-    st = e->own_stream;
-  }
-  struct Rejoin {  // whatever happens below, order the caller's stream after the engine stream
-    bool on; cudaStream_t own, caller; cudaEvent_t ev;
-    ~Rejoin() { if (on) { cudaEventRecord(ev, own); cudaStreamWaitEvent(caller, ev, 0); } }
-  } rejoin{hop, e->own_stream, caller, e->ev_out};
+  Hop hop(e->stream, static_cast<cudaStream_t>(stream), use_graph);
+  if (hop.failed) { set_error("sb_rec_decode_steps: could not create the engine stream"); return -8; }
+  const cudaStream_t st = hop.st;
   if (cudaMemsetAsync(e->st_step, 0, sizeof(int), st) != cudaSuccess ||
       cudaMemsetAsync(e->st_counter, 0, sizeof(unsigned int), st) != cudaSuccess) { cudaGetLastError(); set_error("memset failed"); return -3; }
   if (e->sc_valid && cudaMemsetAsync(e->sc_valid, 0, sizeof(int) * batch, st) != cudaSuccess) { cudaGetLastError(); set_error("memset failed"); return -3; }
@@ -410,34 +343,15 @@ int sb_rec_decode_steps(sb_rec_engine* e, long long* ids_io, const int* slot, in
     for (int i = 0; i < n_steps; ++i) CK(one_step(st));
     return 0;
   }
-  const void* key[8] = {ids_io, slot, pos_io, tok_hist, score_hist, bbox_hist, done_hist, nullptr};
-  bool hit = e->graph_exec && e->graph_batch == batch && std::memcmp(key, e->graph_key, sizeof(key)) == 0;
-  if (!hit) {
-    if (e->graph_exec) { cudaGraphExecDestroy(e->graph_exec); e->graph_exec = nullptr; }
+  const StepGraph::Key key = {ids_io, slot, pos_io, tok_hist, score_hist, bbox_hist, done_hist};
+  if (!e->graph.hit(key, batch)) {
     // one eager step first: sets kernel attributes (not capturable) and validates the launch parameters
     CK(one_step(st));
     n_steps -= 1;
     if (n_steps <= 0) return 0;
-    cudaGraph_t graph = nullptr;
-    cudaError_t cb = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-    if (cb != cudaSuccess) { cudaGetLastError(); set_error("graph capture begin failed: %s", cudaGetErrorString(cb)); return -4; }
-    const long long before = launch_count();
-    int rc = one_step(st);
-    e->graph_nodes = launch_count() - before;
-    count_launches(-e->graph_nodes);  // captured, not executed
-    cudaError_t ce = cudaStreamEndCapture(st, &graph);
-    if (rc || ce != cudaSuccess) { cudaGetLastError(); set_error("graph capture failed: rc=%d %s", rc, cudaGetErrorString(ce)); return -5; }
-    ce = cudaGraphInstantiate(&e->graph_exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) { cudaGetLastError(); set_error("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce)); e->graph_exec = nullptr; return -6; }
-    e->graph_batch = batch;
-    std::memcpy(e->graph_key, key, sizeof(key));
+    CK(e->graph.capture(key, batch, st, one_step));
   }
-  for (int i = 0; i < n_steps; ++i) {
-    if (cudaGraphLaunch(e->graph_exec, st) != cudaSuccess) { cudaGetLastError(); set_error("cudaGraphLaunch failed"); return -7; }
-    count_launches(e->graph_nodes);
-  }
-  return 0;
+  return e->graph.replay(n_steps, st);
 }
 
 int sb_rec_set_sched(sb_rec_engine* e, int* gen_count, long long* ring, unsigned char* row_done, int* n_valid, int* n_active,
@@ -450,7 +364,7 @@ int sb_rec_set_sched(sb_rec_engine* e, int* gen_count, long long* ring, unsigned
   }
   const bool same = e->sc_gen == gen_count && e->sc_ring == ring && e->sc_done == row_done && e->sc_valid == n_valid &&
                     e->sc_active == n_active && e->sc_max_tokens == max_tokens && e->sc_max_repeats == max_repeats;
-  if (!same && e->graph_exec) { cudaGraphExecDestroy(e->graph_exec); e->graph_exec = nullptr; }   // the captured step changes
+  if (!same) e->graph.invalidate();   // the captured step changes
   e->sc_gen = gen_count; e->sc_ring = gen_count ? ring : nullptr; e->sc_done = gen_count ? row_done : nullptr;
   e->sc_valid = gen_count ? n_valid : nullptr; e->sc_active = gen_count ? n_active : nullptr;
   e->sc_max_tokens = gen_count ? max_tokens : 0; e->sc_max_repeats = gen_count ? max_repeats : 0;
