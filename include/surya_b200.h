@@ -283,6 +283,23 @@ int sb_det_normalize_u8(int dtype, const unsigned char* pages_nhwc, void* out_nc
 int sb_det_text_front(int dtype, const void* logits, int n_labels, int B, int hs, int ws, int HO, int WO, void* map16,
                       unsigned char* mask, float* thresholds, unsigned int* hist_scratch, float text_threshold, float low_text,
                       void* stream);
+/* Back half of the detection post-processing on the device (surya/detection/heatmap.py:33-107, detect_boxes after the mask),
+ * fed by sb_det_text_front's map16 [B,H,W] (dtype fp16 / bf16), mask [B,H,W] uint8 and thresholds [B,4]:
+ * cv2.connectedComponentsWithStats(connectivity=4) (components numbered in raster order of their first pixel), the
+ * area >= 10 and peak >= text_threshold filter, and cv2.dilate's output reduced to its leftmost and rightmost pixel per row.
+ * Per page b, for the kept components in label order:
+ *   count[b]                      kept components (also when they exceed the capacity)
+ *   overflow[b]                   1 when count > max_boxes or their points exceed max_points: the tables of that page are
+ *                                 incomplete and it must go through the host path
+ *   box  [B, max_boxes, 7] int32  dilated bounding box x0, y0, x1, y1 (inclusive), point offset, point count, kernel size ks
+ *   peak [B, max_boxes] fp32      largest map value of the component (the 16-bit value widened)
+ *   points [B, max_points, 2] int32  (xl, Y), (xr, Y) for every dilated row Y, top to bottom
+ * cv2.minAreaRect over a box's points equals minAreaRect over every dilated pixel (same hull).
+ * scratch: at least B * (18 * H * W + 8 * H + 4 * max_points + 20) bytes (labels 4 B/px, per-component stats 28 B for at most
+ * ceil(H*W / 2) components, row counts, per-dilated-row extents), no initial contents needed; scratch_bytes is checked. */
+int sb_det_text_boxes(int dtype, const void* map16, const unsigned char* mask, const float* thresholds, int B, int H, int W,
+                      int max_boxes, int max_points, void* scratch, size_t scratch_bytes, int* count, int* overflow, int* box,
+                      float* peak, int* points, void* stream);
 /* parity tap: copy workspace buffer `buf` (NHWC) into dst. */
 int sb_det_debug_copy(sb_det_engine* eng, int buf, void* dst, size_t bytes, void* stream);
 

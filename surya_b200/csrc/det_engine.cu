@@ -190,6 +190,27 @@ int sb_det_text_front(int dtype, const void* logits, int n_labels, int B, int hs
                         low_text, static_cast<cudaStream_t>(stream));
 }
 
+int sb_det_text_boxes(int dtype, const void* map16, const unsigned char* mask, const float* thresholds, int B, int H, int W,
+                      int max_boxes, int max_points, void* scratch, size_t scratch_bytes, int* count, int* overflow, int* box,
+                      float* peak, int* points, void* stream) {
+  if (!map16 || !mask || !thresholds || !scratch || !count || !overflow || !box || !peak || !points) {
+    set_error("sb_det_text_boxes: null argument");
+    return -1;
+  }
+  if (B <= 0 || H <= 0 || W <= 0 || max_boxes <= 0 || max_points < 2) {
+    set_error("sb_det_text_boxes: non-positive size (B=%d H=%d W=%d max_boxes=%d max_points=%d)", B, H, W, max_boxes,
+              max_points);
+    return -1;
+  }
+  const size_t need = det_text_boxes_scratch_bytes(B, H, W, max_points);
+  if (scratch_bytes < need) {
+    set_error("sb_det_text_boxes: scratch of %zu bytes, %zu needed", scratch_bytes, need);
+    return -1;
+  }
+  return det_text_boxes(dtype, map16, mask, thresholds, B, H, W, max_boxes, max_points, scratch, count, overflow, box, peak,
+                        points, static_cast<cudaStream_t>(stream));
+}
+
 int sb_det_debug_copy(sb_det_engine* e, int buf, void* dst, size_t bytes, void* stream) {
   if (!e || buf < 0 || buf >= (int)e->bufs.size()) { set_error("sb_det_debug_copy: bad buffer"); return -1; }
   cudaError_t ce = cudaMemcpyAsync(dst, e->bufs[buf], bytes, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream));

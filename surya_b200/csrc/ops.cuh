@@ -106,6 +106,12 @@ int det_normalize_u8(int dtype, const unsigned char* in, void* out, int B, int H
 // (text_threshold, low_text, top-10 % mean, scaling factor).
 int det_text_front(int dtype, const void* logits, int n_labels, int B, int hs, int ws, int HO, int WO, void* map16,
                    unsigned char* mask, float* thr, unsigned int* hist, float text_threshold, float low_text, cudaStream_t st);
+// Back half on the device (det_boxes.cu): connected components, keep filter and dilated row extents as per-page tables
+// (layout in include/surya_b200.h, sb_det_text_boxes).
+size_t det_text_boxes_scratch_bytes(int B, int H, int W, int max_points);
+int det_text_boxes(int dtype, const void* map16, const unsigned char* mask, const float* thr, int B, int H, int W,
+                   int max_boxes, int max_points, void* scratch, int* count, int* overflow, int* box, float* peak, int* points,
+                   cudaStream_t st);
 
 // Layout / table_rec kernels (layout_ops.cu).
 int layernorm(int dtype, const void* x, const void* w, const void* b, void* y, int rows, int C, float eps, cudaStream_t st);

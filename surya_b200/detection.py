@@ -26,6 +26,21 @@ from .ops import ACT, dt_code
 
 OP_STEM, OP_CONV, OP_PW, OP_DW, OP_GPW, OP_MLA, OP_UPCAT, OP_CLS = range(8)
 
+# Capacity of sb_det_text_boxes' per-page tables: text lines, and points (two per dilated row of each line).  A page beyond
+# either goes through the host path.
+DEFAULT_MAX_BOXES = 1024
+DEFAULT_MAX_POINTS = 65536
+
+
+def box_tables(n: int, max_boxes: int, max_points: int, device=None) -> Dict[str, torch.Tensor]:
+    """Output tables of sb_det_text_boxes for n pages (include/surya_b200.h); pinned host tensors when device is None."""
+    t = {"count": torch.empty((n,), dtype=torch.int32, device=device),
+         "overflow": torch.empty((n,), dtype=torch.int32, device=device),
+         "box": torch.empty((n, max_boxes, 7), dtype=torch.int32, device=device),
+         "peak": torch.empty((n, max_boxes), dtype=torch.float32, device=device),
+         "points": torch.empty((n, max_points, 2), dtype=torch.int32, device=device)}
+    return t if device is not None else {k: v.pin_memory() for k, v in t.items()}
+
 
 class _DetOpC(ctypes.Structure):
     _fields_ = [
@@ -284,6 +299,28 @@ class DetEngine:
               "sb_det_text_front")
         return out
 
+    def text_boxes(self, front: Dict[str, torch.Tensor], max_boxes: int = DEFAULT_MAX_BOXES, max_points: int = DEFAULT_MAX_POINTS,
+                   out: Dict[str, torch.Tensor] | None = None) -> Dict[str, torch.Tensor]:
+        """Back half of detect_boxes (surya/detection/heatmap.py:33-107) on the device (sb_det_text_boxes) for text_front()'s
+        output: connected components, size / peak filter and the dilated row extents as per-page device tables
+        {"count": [B], "overflow": [B], "box": [B, max_boxes, 7] (dilated x0, y0, x1, y1, point offset, point count, ks),
+        "peak": [B, max_boxes], "points": [B, max_points, 2]}.  text_boxes_from_tables() finishes one page on the host."""
+        front = {k: front[k].contiguous() for k in ("map", "mask", "thr")}
+        B, H, W = front["map"].shape
+        dev = front["map"].device
+        if out is None:
+            out = box_tables(B, max_boxes, max_points, device=dev)
+        need = B * (18 * H * W + 8 * H + 4 * max_points + 20)
+        scratch = getattr(self, "_boxes_scratch", None)
+        if scratch is None or scratch.numel() < need:
+            scratch = torch.empty((need,), dtype=torch.uint8, device=dev)
+            self._boxes_scratch = scratch
+        check(self.lib.sb_det_text_boxes(c_int(dt_code(front["map"].dtype)), ptr(front["map"]), ptr(front["mask"]), ptr(front["thr"]),
+                                         c_int(B), c_int(H), c_int(W), c_int(max_boxes), c_int(max_points), ptr(scratch),
+                                         ctypes.c_size_t(scratch.numel()), ptr(out["count"]), ptr(out["overflow"]), ptr(out["box"]),
+                                         ptr(out["peak"]), ptr(out["points"]), stream_ptr()), "sb_det_text_boxes")
+        return out
+
     def debug_buffer(self, name: str, B: int, H: int, W: int, C: int) -> torch.Tensor:
         idx = self.prog.buf_names.index(name)
         out = torch.empty((B, H, W, C), dtype=self.dtype, device=self.device)
@@ -389,12 +426,12 @@ def detect_pages_host(engine: DetEngine, pages_host: torch.Tensor, out_host: tor
     return out_host
 
 
-def detect_text_front_host(engine: DetEngine, pages_host: torch.Tensor, chunk: int = 8, out_size: Tuple[int, int] | None = None,
-                           text_threshold: float = 0.6, low_text: float = 0.35, sync: bool = True):
-    """Host-to-host detection with the post-processing front half on the device: pinned NCHW pages in, per page the 16-bit text
-    map, the binarised mask and the dynamic thresholds out (3 bytes per pixel over PCIe instead of the 8 of two fp32 heat maps;
-    same three-stream pipeline as detect_pages_host).  Returns pinned tensors {"map": [B,H,W], "mask": [B,H,W] u8, "thr": [B,4]};
-    feed them to text_boxes_from_front()."""
+def _front_pipeline(engine: DetEngine, pages_host: torch.Tensor, chunk: int, out_size: Tuple[int, int] | None,
+                    text_threshold: float, low_text: float, sync: bool, tables: Tuple[int, int] | None = None):
+    """Three-stream chunk pipeline of detect_text_front_host / detect_text_boxes_host: the upload of chunk i+1, normalise +
+    forward + sb_det_text_front of chunk i and the download of chunk i-1 run on three streams, so PCIe time hides behind the
+    kernels.  tables=None downloads the text front (map, mask, thresholds); tables=(max_boxes, max_points) runs
+    sb_det_text_boxes after the front and downloads only its tables.  Returns pinned tensors indexed by page."""
     u8 = pages_host.dtype == torch.uint8        # raw pages [B,H,W,3]: normalised on the device (3 bytes per pixel over PCIe)
     if u8:
         B, H, W, _ = pages_host.shape
@@ -403,20 +440,25 @@ def detect_text_front_host(engine: DetEngine, pages_host: torch.Tensor, chunk: i
     size = out_size or (H, W)
     dev = engine.device
     L = engine.cfg.num_labels
-    key = ("front", chunk, H, W, size, pages_host.dtype, B)
-    st = getattr(engine, "_pipe_front", None)
+    key = (chunk, H, W, size, pages_host.dtype, B, tables)
+    attr = "_pipe_front" if tables is None else "_pipe_boxes"
+    st = getattr(engine, attr, None)
     if st is None or st["key"] != key:
+        front = [{"map": torch.empty((chunk, size[0], size[1]), dtype=engine.dtype, device=dev),
+                  "mask": torch.empty((chunk, size[0], size[1]), dtype=torch.uint8, device=dev),
+                  "thr": torch.empty((chunk, 4), dtype=torch.float32, device=dev)} for _ in range(2)]
+        if tables is None:
+            down = front
+            host = {k: torch.empty((B,) + v.shape[1:], dtype=v.dtype).pin_memory() for k, v in front[0].items()}
+        else:
+            down = [box_tables(chunk, *tables, device=dev) for _ in range(2)]
+            host = box_tables(B, *tables)
         st = {"key": key, "s_in": torch.cuda.Stream(dev), "s_c": torch.cuda.Stream(dev), "s_out": torch.cuda.Stream(dev),
               "x": [torch.empty((chunk, H, W, 3) if u8 else (chunk, 3, H, W), dtype=pages_host.dtype, device=dev) for _ in range(2)],
               "xn": [torch.empty((chunk, 3, H, W), dtype=engine.dtype, device=dev) for _ in range(2)] if u8 else None,
               "lg": [torch.empty((chunk, L, H // 4, W // 4), dtype=engine.dtype, device=dev) for _ in range(2)],
-              "o": [{"map": torch.empty((chunk, size[0], size[1]), dtype=engine.dtype, device=dev),
-                     "mask": torch.empty((chunk, size[0], size[1]), dtype=torch.uint8, device=dev),
-                     "thr": torch.empty((chunk, 4), dtype=torch.float32, device=dev)} for _ in range(2)],
-              "host": {"map": torch.empty((B, size[0], size[1]), dtype=engine.dtype).pin_memory(),
-                       "mask": torch.empty((B, size[0], size[1]), dtype=torch.uint8).pin_memory(),
-                       "thr": torch.empty((B, 4), dtype=torch.float32).pin_memory()}}
-        engine._pipe_front = st
+              "front": front, "down": down, "host": host}
+        setattr(engine, attr, st)
     s_in, s_c, s_out = st["s_in"], st["s_c"], st["s_out"]
     host = st["host"]
     cur = torch.cuda.current_stream(dev)
@@ -438,15 +480,16 @@ def detect_text_front_host(engine: DetEngine, pages_host: torch.Tensor, chunk: i
                 s_c.wait_event(ev_o[k])
             xin = engine.normalize_u8(st["x"][k][:n], out=st["xn"][k][:n]) if u8 else st["x"][k][:n]
             engine.forward(xin, out=st["lg"][k][:n])
-            o = st["o"][k]
-            engine.text_front(st["lg"][k][:n], size, text_threshold, low_text,
-                              out={"map": o["map"][:n], "mask": o["mask"][:n], "thr": o["thr"][:n]})
+            front = {name: t[:n] for name, t in st["front"][k].items()}
+            engine.text_front(st["lg"][k][:n], size, text_threshold, low_text, out=front)
+            if tables is not None:
+                engine.text_boxes(front, *tables, out={name: t[:n] for name, t in st["down"][k].items()})
             ev_c[k] = torch.cuda.Event()
             ev_c[k].record(s_c)
         with torch.cuda.stream(s_out):
             s_out.wait_event(ev_c[k])
-            for name in ("map", "mask", "thr"):
-                host[name][b0:b1].copy_(st["o"][k][name][:n], non_blocking=True)
+            for name, t in host.items():
+                t[b0:b1].copy_(st["down"][k][name][:n], non_blocking=True)
             ev_o[k] = torch.cuda.Event()
             ev_o[k].record(s_out)
     cur.wait_stream(s_out)
@@ -456,6 +499,37 @@ def detect_text_front_host(engine: DetEngine, pages_host: torch.Tensor, chunk: i
             if ev is not None:
                 ev.synchronize()
     return host
+
+
+def detect_text_front_host(engine: DetEngine, pages_host: torch.Tensor, chunk: int = 8, out_size: Tuple[int, int] | None = None,
+                           text_threshold: float = 0.6, low_text: float = 0.35, sync: bool = True):
+    """Host-to-host detection with the post-processing front half on the device: pinned NCHW pages (or uint8 NHWC pages) in, per
+    page the 16-bit text map, the binarised mask and the dynamic thresholds out (3 bytes per pixel over PCIe instead of the 8 of
+    two fp32 heat maps; same three-stream pipeline as detect_pages_host).  Returns pinned tensors {"map": [B,H,W],
+    "mask": [B,H,W] u8, "thr": [B,4]}; feed them to text_boxes_from_front()."""
+    return _front_pipeline(engine, pages_host, chunk, out_size, text_threshold, low_text, sync)
+
+
+def detect_text_boxes_host(engine: DetEngine, pages_host: torch.Tensor, chunk: int = 8, out_size: Tuple[int, int] | None = None,
+                           text_threshold: float = 0.6, low_text: float = 0.35, max_boxes: int = DEFAULT_MAX_BOXES,
+                           max_points: int = DEFAULT_MAX_POINTS):
+    """Host-to-host detection with the whole text-box post-processing of detect_boxes (surya/detection/heatmap.py:27-107) on the
+    device except cv2.minAreaRect: pages in as for detect_text_front_host, per page (list of 4x2 float32 boxes, list of
+    confidences) out, equal to text_boxes_from_front on detect_text_front_host's output.  Only the box tables cross PCIe
+    (max_boxes * 32 + max_points * 8 + 8 bytes per page).  A page whose components exceed the table capacity is run again through
+    the text front and finished on the host by text_boxes_from_front.  The host finish runs in the calling thread: it is mostly
+    Python, and a thread pool over the pages was slower."""
+    tabs = _front_pipeline(engine, pages_host, chunk, out_size, text_threshold, low_text, True, (max_boxes, max_points))
+    count, overflow, box, peak, points = (tabs[k].numpy() for k in ("count", "overflow", "box", "peak", "points"))
+    out = [None if overflow[b] else text_boxes_from_tables(box[b], peak[b], points[b], int(count[b])) for b in range(len(count))]
+    over = [b for b in range(len(count)) if overflow[b]]
+    if over:
+        front = detect_text_front_host(engine, pages_host[over].pin_memory(), chunk, out_size, text_threshold, low_text)
+        maps = front["map"] if front["map"].dtype != torch.bfloat16 else front["map"].float()
+        for j, b in enumerate(over):
+            out[b] = text_boxes_from_front(maps[j].numpy(), front["mask"][j].numpy(), float(front["thr"][j, 0]),
+                                           float(front["thr"][j, 1]))
+    return out
 
 
 def text_boxes_from_front(line_map, mask, text_threshold: float, low_text: float):
@@ -498,6 +572,31 @@ def text_boxes_from_front(line_map, mask, text_threshold: float, low_text: float
         max_confidence = max(max_confidence, line_max)
         confidences.append(line_max)
         det.append(box)
+    if max_confidence > 0:
+        confidences = [c / max_confidence for c in confidences]
+    return det, confidences
+
+
+def text_boxes_from_tables(box, peak, points, count: int):
+    """Host finish of one page's sb_det_text_boxes tables: the part of detect_boxes (surya/detection/heatmap.py:53-107) after
+    the dilation, with text_boxes_from_front's types and order.  minAreaRect over two points per dilated row gives the same
+    rectangle as over every dilated pixel; the dilated bounding box is the diamond fix-up's left / right / top / bottom."""
+    import cv2
+    import numpy as np
+
+    det, confidences, max_confidence = [], [], 0
+    for k in range(count):
+        x0, y0, x1, y1, off, n = (int(v) for v in box[k, :6])
+        contours = points[off:off + n].astype(np.int64)       # the dtype np.nonzero gives the host path
+        rect = cv2.boxPoints(cv2.minAreaRect(contours))
+        bw, bh = np.linalg.norm(rect[0] - rect[1]), np.linalg.norm(rect[1] - rect[2])
+        if abs(1 - max(bw, bh) / (min(bw, bh) + 1e-5)) <= 0.1:
+            rect = np.array([[x0, y0], [x1, y0], [x1, y1], [x0, y1]], dtype=np.float32)
+        rect = np.roll(rect, 4 - rect.sum(axis=1).argmin(), 0)
+        line_max = peak[k]
+        max_confidence = max(max_confidence, line_max)
+        confidences.append(line_max)
+        det.append(rect)
     if max_confidence > 0:
         confidences = [c / max_confidence for c in confidences]
     return det, confidences

@@ -2,7 +2,8 @@
 surya/recognition/__init__.py:773-942) on the CUDA engines: detect -> boxes -> crop -> width-sorted recognition.
 
   pages (uint8)  --H2D 3 B/px-->  normalise + EfficientViT + post-processing front half (device)
-                 --D2H 3 B/px-->  connected components / min-area rectangles (host OpenCV, thread pool; heatmap.py:27-107)
+                 connected components, size / peak filter, dilated row extents (device; heatmap.py:33-60)
+                 --D2H tables-->  min-area rectangles over two points per dilated row (host OpenCV; heatmap.py:61-107)
                  polygons      -> y-expansion, clamping, containment filter (heatmap.py:140-175, common/util.py:9-36)
                  line crops    -> polygon-masked slices (input/processing.py:57-101), sorted by width (recognition/__init__.py:848)
                  crops         -> RecognitionRunner (processor mirror on the host, engine prefill / decode on the device)
@@ -15,7 +16,6 @@ Host post-processing here is the minimum the data flow needs; detokenisation / t
 from __future__ import annotations
 
 import time
-from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import shard
-from .detection import DetEngine, detect_text_front_host, text_boxes_from_front
+from .detection import DetEngine, detect_text_boxes_host
 from .recognition import RecEngine, RecognitionRunner
 
 Y_EXPAND_MARGIN = 0.05      # settings.DETECTOR_BOX_Y_EXPAND_MARGIN
@@ -108,7 +108,9 @@ class OcrPipeline:
 
     def __init__(self, det: DetEngine, rec: RecEngine, rec_batch: int = 256, max_tokens: int = 128, det_chunk: int = 16,
                  workers: int = 16, math_mode: bool = True, preprocess: str = "host"):
-        """preprocess: "host" — crops are resized / normalised / tiled by the OpenCV thread pool (the reference's processor code);
+        """workers: no longer used by any step.  The detection boxes are finished in the calling thread, because that measured
+        faster than a thread pool once connected components and dilation moved to the device.
+        preprocess: "host" — crops are resized / normalised / tiled by the OpenCV thread pool (the reference's processor code);
         "device" — uint8 crops go up as they are and sb_rec_preprocess does that work on the GPU (SURVEY §8 f2)."""
         if preprocess not in ("host", "device"):
             raise ValueError("preprocess must be 'host' or 'device'")
@@ -119,18 +121,8 @@ class OcrPipeline:
     def detect(self, pages_u8: torch.Tensor):
         """pinned uint8 [n, H, W, 3] -> per page (polygons, confidences)."""
         n, H, W, _ = pages_u8.shape
-        front = detect_text_front_host(self.det, pages_u8, chunk=self.det_chunk)
-        maps, masks, thr = front["map"].numpy() if front["map"].dtype != torch.bfloat16 else front["map"].float().numpy(), \
-            front["mask"].numpy(), front["thr"].numpy()
-
-        def one(b):
-            boxes, conf = text_boxes_from_front(maps[b], masks[b], float(thr[b, 0]), float(thr[b, 1]))
-            return page_polygons(boxes, conf, (W, H), (W, H))
-
-        if self.workers > 1 and n > 1:
-            with ThreadPoolExecutor(max_workers=min(self.workers, n)) as ex:
-                return list(ex.map(one, range(n)))
-        return [one(b) for b in range(n)]
+        boxes = detect_text_boxes_host(self.det, pages_u8, chunk=self.det_chunk)
+        return [page_polygons(b, c, (W, H), (W, H)) for b, c in boxes]
 
     def run(self, pages: np.ndarray, fixed_steps: bool = False):
         t = {}
