@@ -376,6 +376,12 @@ int sb_bbox_embed_sum(int dtype, const long long* boxes, const void* const* tabl
 int sb_attn_single_query(int dtype, const void* q, int ldq, const void* K, const void* V, long long batch_stride,
                          long long head_stride, long long token_stride, void* out, int ldo, int B, int nh, int nkv, int head_dim,
                          int n_keys, float scale, void* stream);
+/* The same with a row -> K/V-set index: query row b reads the K/V set kv_index[b] (device int32 [B]), so many query rows can
+ * share one set (table_rec cell pass: every row of a table attends to its table's encoder K/V).  Every entry must name a set
+ * that exists behind K / V; the index is a device array and is not range-checked here. */
+int sb_attn_single_query_rows(int dtype, const void* q, int ldq, const void* K, const void* V, long long batch_stride,
+                              long long head_stride, long long token_stride, void* out, int ldo, int B, int nh, int nkv, int head_dim,
+                              int n_keys, float scale, const int* kv_index, void* stream);
 /* LabelEmbedding (table_rec/model/decoder.py:46-73): boxes int64 [n,10]; tables = 13 device pointers (w,h,cx,cy,xskew,yskew,
  * x1,y1,x3,y3 of width box_w; category, merge, colspan of width prop_w); out [n, box_w + prop_w]. */
 int sb_label_embed(int dtype, const long long* boxes, const void* const* tables, void* out, int n, int box_w, int prop_w,
@@ -424,6 +430,10 @@ typedef struct sb_layout_config {
   int n_out_heads, head_n[4];                  /* layout: {label_count}; table: {category, merges, 1 (colspan), is_header} */
   int eos, pad;
   int max_batch, s_max;
+  /* sb_layout_decode_rows capacities (0 = derived from max_batch, the sizes sb_layout_decode uses):
+   *   max_rows            decoder rows and self-attention caches
+   *   max_prefill_tokens  prompt tokens per batched prefill chunk (the decoder activations hold max(max_rows, this) rows) */
+  int max_rows, max_prefill_tokens;
 } sb_layout_config;
 typedef struct sb_layout_engine sb_layout_engine;
 
@@ -439,6 +449,22 @@ int sb_layout_encode(sb_layout_engine* e, const void* pixels, int pixels_f32, in
 int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long long* prompt, int q_len, int n_steps,
                      long long* hist_tok, float* hist_bbox, float* const* hist_heads, unsigned char* hist_done, int use_graph,
                      void* stream);
+/* table_rec two-pass flow (TableRecPredictor.batch_table_recognition, surya/table_rec/__init__.py:134-236).
+ * sb_layout_cross_kv projects the cross-attention K/V of every decoder layer for n_tables <= max_batch encoder states
+ * enc [n_tables, Lk, enc_hidden] and holds them.  sb_layout_decode writes the same buffers: after it runs, the held K/V are
+ * gone and sb_layout_decode_rows fails until sb_layout_cross_kv is called again. */
+int sb_layout_cross_kv(sb_layout_engine* e, const void* enc, int n_tables, void* stream);
+/* Greedy decode of `rows` (<= max_rows) sequences against the held K/V: row r attends to table row_table_host[r] (HOST
+ * int32 [rows], each in [0, n_tables)).  prompt [rows, q_len, ncol] int64 (device): positions 0 .. q_len-2 go through the
+ * decoder as one batched prefill (rows * (q_len-1) GEMM rows, in chunks of at most max(max_rows, max_prefill_tokens) tokens),
+ * then the last prompt token and n_steps - 1 generated tokens are decoded as sb_layout_decode does (graphs of 8 steps).
+ * A row is done from its first step whose category is eos or pad; the loop stops after the first group of steps at which every
+ * row is done.  *n_run_host = number of steps whose histories were written (>= the step at which the last row became done;
+ * n_steps when some row never finishes).  Histories as for sb_layout_decode, with rows in place of batch; hist_done required.
+ * q_len - 1 + n_steps must not exceed s_max.  Table engines only. */
+int sb_layout_decode_rows(sb_layout_engine* e, const int* row_table_host, int rows, const long long* prompt, int q_len, int n_steps,
+                          long long* hist_tok, float* hist_bbox, float* const* hist_heads, unsigned char* hist_done,
+                          int* n_run_host, void* stream);
 
 #ifdef __cplusplus
 }

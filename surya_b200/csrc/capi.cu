@@ -157,6 +157,13 @@ int sb_attn_single_query(int dtype, const void* q, int ldq, const void* K, const
   return attn_single_query(dtype, q, ldq, K, V, batch_stride, head_stride, token_stride, out, ldo, B, nh, nkv, head_dim, n_keys,
                            scale, static_cast<cudaStream_t>(stream));
 }
+int sb_attn_single_query_rows(int dtype, const void* q, int ldq, const void* K, const void* V, long long batch_stride,
+                              long long head_stride, long long token_stride, void* out, int ldo, int B, int nh, int nkv, int head_dim,
+                              int n_keys, float scale, const int* kv_index, void* stream) {
+  if (!kv_index) { set_error("sb_attn_single_query_rows: null kv_index (sb_attn_single_query reads set b for row b)"); return -1; }
+  return attn_single_query(dtype, q, ldq, K, V, batch_stride, head_stride, token_stride, out, ldo, B, nh, nkv, head_dim, n_keys,
+                           scale, static_cast<cudaStream_t>(stream), kv_index);
+}
 int sb_label_embed(int dtype, const long long* boxes, const void* const* tables, void* out, int n, int box_w, int prop_w,
                    int bbox_size, int vocab, void* stream) {
   return label_embed(dtype, boxes, tables, out, n, box_w, prop_w, bbox_size, vocab, static_cast<cudaStream_t>(stream));

@@ -36,15 +36,33 @@ struct sb_layout_engine {
   std::vector<void*> ckv, kc, vc;      // per decoder layer
   int* slot = nullptr;
   long long* tok = nullptr;            // [B, ncol]
-  int* pos = nullptr;                  // [B]
-  int* base = nullptr;                 // [1]
+  int* pos = nullptr;                  // [R]
+  int* base = nullptr;                 // [1] + the row-decode state below, carved from the same block
   float* out_bbox = nullptr;           // [B, 6]
   float* out_head[4] = {nullptr, nullptr, nullptr, nullptr};
   unsigned char* done = nullptr;
   int Lk = 0;
+  // sb_layout_decode_rows state (inside the `base` block): active-row count, row -> table map, per-token prefill arrays
+  // (position, cache slot, K/V set; sequence starts and lengths for attn_varlen) and the sticky done flags
+  int *n_active = nullptr, *row_table = nullptr, *t_pos = nullptr, *t_slot = nullptr, *t_kv = nullptr, *t_start = nullptr,
+      *t_len = nullptr;
+  unsigned char* sticky = nullptr;
+  int R = 0, P = 0;                    // decoder rows, decoder activation rows (prefill tokens per chunk)
+  // held cross K/V: sb_layout_cross_kv stamps held_gen = ++kv_gen; sb_layout_decode bumps kv_gen (it overwrites ckv)
+  unsigned long long kv_gen = 0, held_gen = 0;
+  int held_tables = 0;
+  int* h_active = nullptr;             // pinned [2]: active counts of the last two step groups
+  cudaEvent_t ev_active[2] = {nullptr, nullptr};
   // decode loop: GRAPH_GROUP steps per replay, and one step for the tail
   StepGraph g_group{"sb_layout_decode", GRAPH_GROUP}, g_one{"sb_layout_decode", 1};
+  StepGraph g_rows{"sb_layout_decode_rows", GRAPH_GROUP}, g_rows_one{"sb_layout_decode_rows", 1};
   EngineStream stream;
+
+  ~sb_layout_engine() {
+    for (cudaEvent_t ev : ev_active)
+      if (ev) cudaEventDestroy(ev);
+    if (h_active) cudaFreeHost(h_active);
+  }
 
   int ncol() const { return 6 + c.n_out_heads; }
   // ---- weight table (see include/surya_b200.h)
@@ -124,8 +142,14 @@ static int run_encoder(sb_layout_engine* e, const void* pixels, int is_f32, int 
 }
 
 // ------------------------------------------------------------------------------------------------ ADETR decoder
-// One q_len = 1 call on the persistent state: embedding of e->tok rows -> layers -> heads into e->out_*.
-static int run_token(sb_layout_engine* e, const long long* tok, const int* pos, int B, cudaStream_t st) {
+// Batched prompt prefill of sb_layout_decode_rows: the B token rows are n_seq sequences of len tokens each; self-attention is
+// RoPE + cache append at (t_pos, t_slot) and causal attention within each sequence, and nothing after the last layer runs.
+struct Prefill { int n_seq, len; };
+
+// One q_len = 1 call on the persistent state: embedding of e->tok rows -> layers -> heads into e->out_*.  kv_index: row b reads
+// the cross K/V of table kv_index[b] (null: table b).  pf: the rows are prompt tokens (see Prefill) instead of decode steps.
+static int run_token(sb_layout_engine* e, const long long* tok, const int* pos, int B, cudaStream_t st,
+                     const int* kv_index = nullptr, const Prefill* pf = nullptr) {
   const sb_layout_config& c = e->c;
   const int dt = c.dtype, Hd = c.hidden, nh = c.n_heads, nkv = c.n_kv, hd = c.head_dim;
   const float scale = 1.0f / sqrtf(static_cast<float>(hd));
@@ -140,18 +164,30 @@ static int run_token(sb_layout_engine* e, const long long* tok, const int* pos, 
     CK(gemm_launch(weight_gemm(dt, e->dn, Hd, e->WD(l, SB_LWD_CQ_W), Hd, e->dq, nh * hd, B, nh * hd, Hd, nullptr), st));
     const uint8_t* kv = static_cast<const uint8_t*>(e->ckv[l]);
     CK(attn_single_query(dt, e->dq, nh * hd, kv, kv + static_cast<size_t>(nkv) * hd * e->esz, static_cast<long long>(e->Lk) * KVW, hd,
-                         KVW, e->da, nh * hd, B, nh, nkv, hd, e->Lk, scale, st));
+                         KVW, e->da, nh * hd, B, nh, nkv, hd, e->Lk, scale, st, kv_index));
     CK(gemm_launch(weight_gemm(dt, e->da, nh * hd, e->WD(l, SB_LWD_CO_W), nh * hd, e->dcross, Hd, B, Hd, nh * hd, e->WD(l, SB_LWD_CO_B),
                                e->dx, Hd), st));
     // causal self attention (RoPE + cache append fused into the attention kernel)
     CK(rmsnorm(dt, e->dcross, Hd, e->WD(l, SB_LWD_SELF_NORM), e->dn, Hd, B, Hd, c.rms_eps, nullptr, st, 1));
     CK(gemm_launch(weight_gemm(dt, e->dn, Hd, e->WD(l, SB_LWD_SQKV_W), Hd, e->dqkv, QW, B, QW, Hd, nullptr), st));
-    DecodeAttnArgs a;
-    a.dtype = dt; a.qkv = e->dqkv; a.ld = QW; a.kcache = e->kc[l]; a.vcache = e->vc[l]; a.slot = e->slot; a.pos = pos;
-    a.inv_freq = static_cast<const float*>(e->WX(SB_LWX_INV_FREQ));
-    a.out = e->da; a.ldo = nh * hd; a.batch = B; a.n_heads = nh; a.n_kv_heads = nkv; a.head_dim = hd; a.s_max = c.s_max;
-    a.scale = scale;
-    CK(decode_attn(a, st));
+    if (pf) {
+      CK(rope_kv_append(dt, e->dqkv, QW, e->t_pos, e->t_slot, static_cast<const float*>(e->WX(SB_LWX_INV_FREQ)), e->kc[l], e->vc[l],
+                        B, nh, nkv, hd, c.s_max, st));
+      const uint8_t* qkv = static_cast<const uint8_t*>(e->dqkv);
+      AttnArgs a;
+      a.dtype = dt; a.q = qkv; a.ldq = QW; a.k = qkv + static_cast<size_t>(nh) * hd * e->esz; a.ldk = QW;
+      a.v = qkv + static_cast<size_t>(nh + nkv) * hd * e->esz; a.ldv = QW; a.out = e->da; a.ldo = nh * hd;
+      a.seq_start = e->t_start; a.seq_len = e->t_len; a.n_seq = pf->n_seq; a.max_len = pf->len;
+      a.n_heads = nh; a.n_kv_heads = nkv; a.head_dim = hd; a.causal = 1; a.scale = scale;
+      CK(attn_varlen(a, st));
+    } else {
+      DecodeAttnArgs a;
+      a.dtype = dt; a.qkv = e->dqkv; a.ld = QW; a.kcache = e->kc[l]; a.vcache = e->vc[l]; a.slot = e->slot; a.pos = pos;
+      a.inv_freq = static_cast<const float*>(e->WX(SB_LWX_INV_FREQ));
+      a.out = e->da; a.ldo = nh * hd; a.batch = B; a.n_heads = nh; a.n_kv_heads = nkv; a.head_dim = hd; a.s_max = c.s_max;
+      a.scale = scale;
+      CK(decode_attn(a, st));
+    }
     const void* res_src = c.double_residual ? e->dx : e->dcross;
     CK(gemm_launch(weight_gemm(dt, e->da, nh * hd, e->WD(l, SB_LWD_SO_W), nh * hd, e->dres, Hd, B, Hd, nh * hd, e->WD(l, SB_LWD_SO_B),
                                res_src, Hd), st));
@@ -163,6 +199,7 @@ static int run_token(sb_layout_engine* e, const long long* tok, const int* pos, 
     down.allow_splitk = 1;
     CK(gemm_launch(down, st));
   }
+  if (pf) return 0;        // the prompt's K/V are cached; its last token runs as the first decode step
   CK(rmsnorm(dt, e->dx, Hd, e->WX(SB_LWX_FINAL_NORM), e->dn, Hd, B, Hd, c.rms_eps, nullptr, st, 1));
   CK(layernorm(dt, e->dn, e->WX(SB_LWX_OUT_LN_W), e->WX(SB_LWX_OUT_LN_B), e->dh, B, Hd, c.dec_ln_eps, st));
   const int hb = e->dec_base() + e->n_tables() + c.dec_layers * SB_LW_DEC_LAYER + SB_LW_DEC_TAIL;
@@ -216,7 +253,20 @@ int sb_layout_create(const sb_layout_config* cfg, const void* const* weights, in
     if (!weights[i]) { set_error("sb_layout_create: weight pointer %d is null", i); delete e; return -4; }
   e->w.assign(weights, weights + n_weights);
   const size_t es = e->esz;
+  if (c.max_batch < 1 || c.max_rows < 0 || c.max_prefill_tokens < 0 || c.s_max < 1) {
+    set_error("sb_layout_create: max_batch (%d) and s_max (%d) must be positive, max_rows (%d) and max_prefill_tokens (%d) not negative",
+              c.max_batch, c.s_max, c.max_rows, c.max_prefill_tokens);
+    delete e;
+    return -2;
+  }
   const size_t B = c.max_batch;
+  // decoder rows (self-attention caches) and activation rows, never fewer than max_batch; 0 keeps the sizes sb_layout_decode has
+  // always used
+  const size_t R = static_cast<size_t>(c.max_rows) > B ? static_cast<size_t>(c.max_rows) : B;
+  size_t P = R;
+  if (static_cast<size_t>(c.max_prefill_tokens) > P) P = c.max_prefill_tokens;
+  e->R = static_cast<int>(R);
+  e->P = static_cast<int>(P);
   const size_t rows0 = B * (c.img_h / c.patch) * (c.img_w / c.patch);
   const size_t C0 = c.embed_dim;
   const int K0 = c.in_ch * c.patch * c.patch, Kp = (K0 + 63) / 64 * 64;
@@ -225,18 +275,21 @@ int sb_layout_create(const sb_layout_config* cfg, const void* const* weights, in
   for (int s = 0; s < c.n_stages - 1; ++s) { Hl /= 2; Wl /= 2; }
   const size_t Lk = static_cast<size_t>(Hl) * Wl;
   const size_t Hd = c.hidden, QW = (c.n_heads + 2 * c.n_kv) * c.head_dim, KVW = 2 * c.n_kv * c.head_dim;
-  const size_t cache = B * c.n_kv * c.s_max * c.head_dim * es;
+  const size_t cache = R * c.n_kv * c.s_max * c.head_dim * es;
   const size_t QH = static_cast<size_t>(c.n_heads) * c.head_dim;
   Arena& a = e->arena;
   a.add(e->x, rows0 * C0 * es); a.add(e->h, rows0 * hcols * es); a.add(e->qkv, rows0 * 3 * C0 * es); a.add(e->ao, rows0 * C0 * es);
   a.add(e->mlp, rows0 * 4 * C0 * es);
-  a.add(e->dx, B * Hd * es); a.add(e->dn, B * Hd * es); a.add(e->dq, B * QH * es); a.add(e->da, B * QH * es);
-  a.add(e->dcross, B * Hd * es); a.add(e->dres, B * Hd * es); a.add(e->dqkv, B * QW * es); a.add(e->dm, B * c.inter * es);
-  a.add(e->dh, B * Hd * es);
+  a.add(e->dx, P * Hd * es); a.add(e->dn, P * Hd * es); a.add(e->dq, P * QH * es); a.add(e->da, P * QH * es);
+  a.add(e->dcross, P * Hd * es); a.add(e->dres, P * Hd * es); a.add(e->dqkv, P * QW * es); a.add(e->dm, P * c.inter * es);
+  a.add(e->dh, R * Hd * es);
   a.add(e->enc, B * Lk * c.enc_hidden * es);
-  a.add(e->slot, B * sizeof(int)); a.add(e->tok, B * 10 * sizeof(long long)); a.add(e->pos, B * sizeof(int)); a.add(e->base, 256);
-  a.add(e->out_bbox, B * 6 * sizeof(float)); a.add(e->done, B);
-  for (int k = 0; k < 4; ++k) a.add(e->out_head[k], B * (k < c.n_out_heads ? c.head_n[k] : 1) * sizeof(float));
+  // `base` block: [0] history base, [1] active-row count, [2..3] spare, then row_table [R], five per-token arrays [P], sticky [R]
+  const size_t state = (4 + R + 5 * P) * sizeof(int) + R;
+  a.add(e->slot, R * sizeof(int)); a.add(e->tok, P * 10 * sizeof(long long)); a.add(e->pos, R * sizeof(int));
+  a.add(e->base, state > 256 ? state : 256);
+  a.add(e->out_bbox, R * 6 * sizeof(float)); a.add(e->done, R);
+  for (int k = 0; k < 4; ++k) a.add(e->out_head[k], R * (k < c.n_out_heads ? c.head_n[k] : 1) * sizeof(float));
   e->ckv.resize(c.dec_layers); e->kc.resize(c.dec_layers); e->vc.resize(c.dec_layers);
   for (int l = 0; l < c.dec_layers; ++l) { a.add(e->ckv[l], B * Lk * KVW * es); a.add(e->kc[l], cache); a.add(e->vc[l], cache); }
   if (a.alloc() != cudaSuccess) {
@@ -244,9 +297,13 @@ int sb_layout_create(const sb_layout_config* cfg, const void* const* weights, in
     delete e;
     return -5;
   }
-  std::vector<int> slots(B);
-  for (size_t i = 0; i < B; ++i) slots[i] = static_cast<int>(i);
-  cudaMemcpy(e->slot, slots.data(), B * sizeof(int), cudaMemcpyHostToDevice);
+  e->n_active = e->base + 1;
+  e->row_table = e->base + 4;
+  e->t_pos = e->row_table + R; e->t_slot = e->t_pos + P; e->t_kv = e->t_slot + P; e->t_start = e->t_kv + P; e->t_len = e->t_start + P;
+  e->sticky = reinterpret_cast<unsigned char*>(e->t_len + P);
+  std::vector<int> slots(R);
+  for (size_t i = 0; i < R; ++i) slots[i] = static_cast<int>(i);
+  cudaMemcpy(e->slot, slots.data(), R * sizeof(int), cudaMemcpyHostToDevice);
   e->Lk = static_cast<int>(Lk);
   *out = e;
   return 0;
@@ -275,6 +332,7 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
 
   const int B = batch, ncol = e->ncol();
   const size_t es = e->esz;
+  ++e->kv_gen;                     // the K/V held by sb_layout_cross_kv are overwritten below
   // encoder states -> persistent buffer; cross-attention K/V of every layer (SuryaADETRDecoderSdpaCrossAttention caches them at
   // the first call, adetr/decoder.py:150-194)
   if (cudaMemcpyAsync(e->enc, enc, static_cast<size_t>(B) * e->Lk * c.enc_hidden * es, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
@@ -325,6 +383,151 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
   }
   CK(e->g_group.replay(left / GRAPH_GROUP, st));
   return e->g_one.replay(left % GRAPH_GROUP, st);
+}
+
+int sb_layout_cross_kv(sb_layout_engine* e, const void* enc, int n_tables, void* stream) {
+  if (!e || !enc) { set_error("sb_layout_cross_kv: null argument"); return -1; }
+  const sb_layout_config& c = e->c;
+  if (n_tables <= 0 || n_tables > c.max_batch) {
+    set_error("sb_layout_cross_kv: %d tables need max_batch >= %d (engine has %d)", n_tables, n_tables, c.max_batch);
+    return -2;
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int KVW = 2 * c.n_kv * c.head_dim;
+  e->held_gen = 0;                 // a failed projection leaves nothing held
+  for (int l = 0; l < c.dec_layers; ++l)
+    CK(gemm_launch(weight_gemm(c.dtype, enc, c.enc_hidden, e->WD(l, SB_LWD_CKV_W), c.enc_hidden, e->ckv[l], KVW, n_tables * e->Lk, KVW,
+                               c.enc_hidden, nullptr), st));
+  e->held_gen = ++e->kv_gen;
+  e->held_tables = n_tables;
+  return 0;
+}
+
+int sb_layout_decode_rows(sb_layout_engine* e, const int* row_table_host, int rows, const long long* prompt, int q_len, int n_steps,
+                          long long* hist_tok, float* hist_bbox, float* const* hist_heads, unsigned char* hist_done,
+                          int* n_run_host, void* stream) {
+  if (!e || !row_table_host || !prompt || !hist_tok || !hist_done || !n_run_host) {
+    set_error("sb_layout_decode_rows: null argument");
+    return -1;
+  }
+  *n_run_host = 0;
+  const sb_layout_config& c = e->c;
+  if (c.kind != 1) { set_error("sb_layout_decode_rows: needs a table_rec engine (done is the category head)"); return -2; }
+  if (e->held_gen == 0 || e->held_gen != e->kv_gen) {
+    set_error("sb_layout_decode_rows: no cross K/V held (sb_layout_decode overwrote them, or sb_layout_cross_kv was not called)");
+    return -3;
+  }
+  if (rows <= 0 || rows > e->R) { set_error("sb_layout_decode_rows: %d rows need max_rows >= %d (engine has %d)", rows, rows, e->R); return -2; }
+  if (q_len < 1 || n_steps < 1 || q_len - 1 + n_steps > c.s_max) {
+    set_error("sb_layout_decode_rows: a %d-token prompt and %d steps need s_max >= %d (engine has %d)", q_len, n_steps,
+              q_len - 1 + n_steps, c.s_max);
+    return -2;
+  }
+  if (q_len - 1 > e->P) {
+    set_error("sb_layout_decode_rows: a %d-token prompt needs max_prefill_tokens >= %d (engine prefills %d tokens per chunk)", q_len,
+              q_len - 1, e->P);
+    return -2;
+  }
+  for (int r = 0; r < rows; ++r)
+    if (row_table_host[r] < 0 || row_table_host[r] >= e->held_tables) {
+      set_error("sb_layout_decode_rows: row %d maps to table %d, outside the %d held tables", r, row_table_host[r], e->held_tables);
+      return -4;
+    }
+  if (!e->h_active) {
+    if (cudaHostAlloc(&e->h_active, 2 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError(); e->h_active = nullptr; set_error("sb_layout_decode_rows: pinned allocation failed"); return -8;
+    }
+    for (cudaEvent_t& ev : e->ev_active)
+      if (!ev && cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
+        cudaGetLastError(); ev = nullptr; set_error("sb_layout_decode_rows: event creation failed"); return -8;
+      }
+  }
+  Hop hop(e->stream, static_cast<cudaStream_t>(stream), true);
+  if (hop.failed) { set_error("sb_layout_decode_rows: could not create the engine stream"); return -8; }
+  const cudaStream_t st = hop.st;
+  const int ncol = e->ncol();
+  const size_t tokb = static_cast<size_t>(ncol) * sizeof(long long);
+
+  // host state, all copied before the one synchronisation below (the copies read pageable memory)
+  const int nq = q_len - 1;                          // prompt tokens that only fill the self-attention caches
+  const int per = nq > 0 ? e->P / nq : 0;            // rows per prefill chunk
+  const int n_chunks = nq > 0 ? (rows + per - 1) / per : 0;
+  std::vector<int> hstate(4 + rows);
+  hstate[0] = q_len - 1;                             // history base: the step at position q_len-1 is history row 0
+  hstate[1] = rows;
+  for (int r = 0; r < rows; ++r) hstate[4 + r] = row_table_host[r];
+  std::vector<int> hpos(rows, q_len - 1);
+  std::vector<int> htok(static_cast<size_t>(n_chunks) * 5 * e->P);
+  auto fail = [](const char* what) { cudaGetLastError(); set_error("sb_layout_decode_rows: %s failed", what); return -5; };
+  if (cudaMemcpyAsync(e->base, hstate.data(), hstate.size() * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+      cudaMemsetAsync(e->sticky, 0, rows, st) != cudaSuccess)
+    return fail("state copy");
+
+  // batched prefill of positions 0 .. q_len-2, chunk by chunk (rows * nq tokens per chunk <= P)
+  for (int ch = 0; ch < n_chunks; ++ch) {
+    const int r0 = ch * per, n = rows - r0 < per ? rows - r0 : per, T = n * nq;
+    int* h = htok.data() + static_cast<size_t>(ch) * 5 * e->P;
+    for (int t = 0; t < T; ++t) {
+      const int r = r0 + t / nq;
+      h[t] = t % nq; h[e->P + t] = r; h[2 * e->P + t] = row_table_host[r];
+    }
+    for (int i = 0; i < n; ++i) { h[3 * e->P + i] = i * nq; h[4 * e->P + i] = nq; }
+    if (cudaMemcpyAsync(e->t_pos, h, 5 * e->P * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpy2DAsync(e->tok, nq * tokb, prompt + static_cast<size_t>(r0) * q_len * ncol, q_len * tokb, nq * tokb, n,
+                          cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+      return fail("prefill copy");
+    const Prefill pf{n, nq};
+    CK(run_token(e, e->tok, nullptr, T, st, e->t_kv, &pf));
+  }
+  // last prompt token of every row -> the first decode step
+  if (cudaMemcpy2DAsync(e->tok, tokb, prompt + static_cast<size_t>(nq) * ncol, q_len * tokb, tokb, rows, cudaMemcpyDeviceToDevice,
+                        st) != cudaSuccess ||
+      cudaMemcpyAsync(e->pos, hpos.data(), rows * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess)
+    return fail("prompt copy");
+  cudaStreamSynchronize(st);       // host sources above are vector memory
+
+  auto body = [&](cudaStream_t s) -> int {
+    CK(run_token(e, e->tok, e->pos, rows, s, e->row_table));
+    CK(run_next(e, rows, n_steps, hist_tok, hist_bbox, hist_heads, hist_done, s));
+    return rows_done_count(e->done, e->sticky, e->n_active, rows, s);
+  };
+  CK(body(st));                    // first step eagerly (sets kernel attributes before any capture)
+  int ran = 1;
+  const int left = n_steps - 1;
+  if (left > 0) {
+    const StepGraph::Key key = {hist_tok, hist_bbox, hist_done, hist_heads ? hist_heads[0] : nullptr,
+                                reinterpret_cast<const void*>(static_cast<uintptr_t>(n_steps))};
+    if (!e->g_rows.hit(key, rows) || !e->g_rows_one.hit(key, rows)) {
+      CK(e->g_rows.capture(key, rows, st, body));
+      CK(e->g_rows_one.capture(key, rows, st, body));
+    }
+    // Early exit: after each group the active-row count goes to pinned memory.  Group g+1 is enqueued before the count of group g
+    // is read, so the GPU never waits for the host; when that count is 0, group g+1's steps are extra and the loop stops.
+    const int groups = left / GRAPH_GROUP;
+    bool stop = false;
+    auto post = [&](int g) -> int {
+      if (cudaMemcpyAsync(e->h_active + (g & 1), e->n_active, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+          cudaEventRecord(e->ev_active[g & 1], st) != cudaSuccess)
+        return fail("active-count copy");
+      return 0;
+    };
+    auto all_done = [&](int g) { cudaEventSynchronize(e->ev_active[g & 1]); return e->h_active[g & 1] == 0; };
+    for (int g = 0; g < groups && !stop; ++g) {
+      CK(e->g_rows.replay(1, st));
+      ran += GRAPH_GROUP;
+      CK(post(g));
+      if (g > 0 && all_done(g - 1)) stop = true;
+    }
+    if (!stop && left % GRAPH_GROUP) {
+      if (groups > 0 && all_done(groups - 1)) stop = true;
+      if (!stop) {
+        CK(e->g_rows_one.replay(left % GRAPH_GROUP, st));
+        ran += left % GRAPH_GROUP;
+      }
+    }
+  }
+  *n_run_host = ran;
+  return 0;
 }
 
 }  // extern "C"

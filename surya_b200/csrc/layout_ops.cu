@@ -485,12 +485,13 @@ int bbox_embed_sum(int dtype, const long long* boxes, const void* const* tables,
 }
 
 // ------------------------------------------------------------------------------------------------ single-query attention
-// q [B, nh*HD]; K/V element (b, kvh, j, c) at base + b*bs + kvh*hs + j*ts + c; out [B, nh*HD]. One CTA per (b, kv head).
+// q [B, nh*HD]; K/V element (set, kvh, j, c) at base + set*bs + kvh*hs + j*ts + c with set = kv_index ? kv_index[b] : b;
+// out [B, nh*HD]. One CTA per (b, kv head).
 template <typename T, int HD, int G>
 __global__ void __launch_bounds__(128) attn_single_query_kernel(const T* __restrict__ q, int ldq, const T* __restrict__ K,
                                                                 const T* __restrict__ V, long long bs, long long hs,
                                                                 long long ts, T* __restrict__ out, int ldo, int n_keys,
-                                                                float scale) {
+                                                                float scale, const int* __restrict__ kv_index) {
   constexpr int VPR = HD / 8, NKG = 128 / VPR;
   extern __shared__ __align__(16) uint8_t smem_sq[];
   T* q_t = reinterpret_cast<T*>(smem_sq);            // [G][HD] query rows, kept in T (first G*HD floats' worth of space)
@@ -501,8 +502,9 @@ __global__ void __launch_bounds__(128) attn_single_query_kernel(const T* __restr
   const int b = blockIdx.x, kvh = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const T* qr = q + static_cast<size_t>(b) * ldq + kvh * G * HD;
   for (int i = tid; i < G * HD; i += 128) q_t[i] = qr[i];
-  const T* kb = K + b * bs + kvh * hs;
-  const T* vb = V + b * bs + kvh * hs;
+  const long long set = kv_index ? kv_index[b] : b;     // K/V set of this query row (many rows may share one set)
+  const T* kb = K + set * bs + kvh * hs;
+  const T* vb = V + set * bs + kvh * hs;
   __syncthreads();
   float tmax[G];
 #pragma unroll
@@ -614,7 +616,7 @@ __global__ void __launch_bounds__(128) attn_single_query_kernel(const T* __restr
 
 template <typename T, int G>
 static int launch_sq(const void* q, int ldq, const void* K, const void* V, long long bs, long long hs, long long ts, void* out,
-                     int ldo, int B, int nkv, int n_keys, float scale, cudaStream_t st) {
+                     int ldo, int B, int nkv, int n_keys, float scale, const int* kv_index, cudaStream_t st) {
   constexpr int HD = 64, NKG = 128 / (HD / 8);
   const size_t smem = (static_cast<size_t>(G) * HD + static_cast<size_t>(NKG) * G * HD + static_cast<size_t>(G) * n_keys) * sizeof(float);
   auto kern = attn_single_query_kernel<T, HD, G>;
@@ -627,20 +629,22 @@ static int launch_sq(const void* q, int ldq, const void* K, const void* V, long 
     }
     attr = smem;
   }
-  kern<<<dim3(B, nkv), 128, smem, st>>>((const T*)q, ldq, (const T*)K, (const T*)V, bs, hs, ts, (T*)out, ldo, n_keys, scale);
+  kern<<<dim3(B, nkv), 128, smem, st>>>((const T*)q, ldq, (const T*)K, (const T*)V, bs, hs, ts, (T*)out, ldo, n_keys, scale,
+                                        kv_index);
   return launch_ok();
 }
 
 int attn_single_query(int dtype, const void* q, int ldq, const void* K, const void* V, long long bs, long long hs, long long ts,
-                      void* out, int ldo, int B, int nh, int nkv, int head_dim, int n_keys, float scale, cudaStream_t st) {
+                      void* out, int ldo, int B, int nh, int nkv, int head_dim, int n_keys, float scale, cudaStream_t st,
+                      const int* kv_index) {
   if (head_dim != 64) { set_error("attn_single_query: head_dim 64 is instantiated (got %d)", head_dim); return -1; }
   if (nkv <= 0 || nh % nkv) { set_error("attn_single_query: nh (%d) must be a positive multiple of nkv (%d)", nh, nkv); return -1; }
   if (n_keys <= 0) { set_error("attn_single_query: n_keys must be positive (got %d)", n_keys); return -1; }
   const int G = nh / nkv;
 #define SQ(T_) \
-  (G == 1 ? launch_sq<T_, 1>(q, ldq, K, V, bs, hs, ts, out, ldo, B, nkv, n_keys, scale, st) : \
-   G == 2 ? launch_sq<T_, 2>(q, ldq, K, V, bs, hs, ts, out, ldo, B, nkv, n_keys, scale, st) : \
-   G == 4 ? launch_sq<T_, 4>(q, ldq, K, V, bs, hs, ts, out, ldo, B, nkv, n_keys, scale, st) : -9)
+  (G == 1 ? launch_sq<T_, 1>(q, ldq, K, V, bs, hs, ts, out, ldo, B, nkv, n_keys, scale, kv_index, st) : \
+   G == 2 ? launch_sq<T_, 2>(q, ldq, K, V, bs, hs, ts, out, ldo, B, nkv, n_keys, scale, kv_index, st) : \
+   G == 4 ? launch_sq<T_, 4>(q, ldq, K, V, bs, hs, ts, out, ldo, B, nkv, n_keys, scale, kv_index, st) : -9)
   int rc = dtype == DT_F16 ? SQ(__half) : SQ(__nv_bfloat16);
 #undef SQ
   if (rc == -9) set_error("attn_single_query: GQA group %d not instantiated (1/2/4)", G);
@@ -769,6 +773,32 @@ int box_next_token(const float* bbox, const float* const* heads, const int* head
   }
   box_next_token_kernel<<<(B + 63) / 64, 64, 0, st>>>(bbox, h, n_heads, bbox_size, out, done, done_head, eos, pad, B, cache_pos,
                                                       hist_base, hist_T, hist_tok, hist_bbox, hist_done);
+  return launch_ok();
+}
+
+// ------------------------------------------------------------------------------------------------ sticky done + active count
+// The stop rule of TableRecPredictor.inference_loop (table_rec/__init__.py:111-115) on the device: sticky[b] |= done[b], and
+// n_active[0] = the number of rows not yet done.  One CTA, so that the count is written by one store after the block reduce.
+__global__ void __launch_bounds__(256) rows_done_count_kernel(const unsigned char* __restrict__ done, unsigned char* __restrict__ sticky,
+                                                              int* __restrict__ n_active, int B) {
+  __shared__ int s_cnt;
+  if (threadIdx.x == 0) s_cnt = 0;
+  __syncthreads();
+  int cnt = 0;
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const unsigned char d = sticky[b] | done[b];
+    sticky[b] = d;
+    cnt += d ? 0 : 1;
+  }
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s_cnt, cnt);
+  __syncthreads();
+  if (threadIdx.x == 0) n_active[0] = s_cnt;
+}
+
+int rows_done_count(const unsigned char* done, unsigned char* sticky, int* n_active, int B, cudaStream_t st) {
+  if (B <= 0) return 0;
+  rows_done_count_kernel<<<1, 256, 0, st>>>(done, sticky, n_active, B);
   return launch_ok();
 }
 

@@ -122,14 +122,18 @@ int swin_window_attn(int dtype, const void* qkv, const float* qkv_bias, const vo
                      int nh, int shift, cudaStream_t st);
 int bbox_embed_sum(int dtype, const long long* boxes, const void* const* tables, void* out, int n, int Hd, int bbox_size,
                    cudaStream_t st);
+// kv_index (device, may be null): query row b reads K/V set kv_index[b] instead of set b.
 int attn_single_query(int dtype, const void* q, int ldq, const void* K, const void* V, long long bs, long long hs, long long ts,
-                      void* out, int ldo, int B, int nh, int nkv, int head_dim, int n_keys, float scale, cudaStream_t st);
+                      void* out, int ldo, int B, int nh, int nkv, int head_dim, int n_keys, float scale, cudaStream_t st,
+                      const int* kv_index = nullptr);
 int label_embed(int dtype, const long long* boxes, const void* const* tables, void* out, int n, int box_w, int prop_w,
                 int bbox_size, int vocab, cudaStream_t st);
 int box_next_token(const float* bbox, const float* const* heads, const int* head_n, const int* head_mode, int n_heads,
                    float bbox_size, long long* out, unsigned char* done, int done_head, int eos, int pad, int B, int* cache_pos,
                    const int* hist_base, int hist_T, long long* hist_tok, float* hist_bbox, float* const* hist_heads,
                    unsigned char* hist_done, cudaStream_t st);
+// sticky[b] |= done[b]; n_active[0] = number of rows b < B with sticky[b] == 0 (table_rec early exit).
+int rows_done_count(const unsigned char* done, unsigned char* sticky, int* n_active, int B, cudaStream_t st);
 
 // Recognition crop preprocessing on the device (preproc.cu): uint8 crops -> Lanczos4 scale_to_fit -> cubic resize to x28 -> normalise ->
 // merge-block-major fp32 tiles.  desc: n_crops x 9 int32 on the device; mean / std3: 3 host floats each.

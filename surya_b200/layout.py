@@ -39,6 +39,7 @@ class _LayoutCfgC(ctypes.Structure):
         ("n_out_heads", ctypes.c_int), ("head_n", ctypes.c_int * 4),
         ("eos", ctypes.c_int), ("pad", ctypes.c_int),
         ("max_batch", ctypes.c_int), ("s_max", ctypes.c_int),
+        ("max_rows", ctypes.c_int), ("max_prefill_tokens", ctypes.c_int),
     ]
 
 
@@ -59,11 +60,15 @@ class LayoutEngine:
 
     def __init__(self, cfg: LayoutConfig, sd_enc: Dict[str, torch.Tensor], sd_dec: Dict[str, torch.Tensor],
                  dtype: torch.dtype = torch.float16, device: str | torch.device = "cuda", max_batch: int = 16,
-                 impl: str = "native"):
+                 impl: str = "native", s_max: Optional[int] = None, max_rows: int = 0, max_prefill_tokens: int = 0):
         """impl = "native": layer loops, workspaces and the decode loop run inside libsurya_b200.so (sb_layout_*);
         impl = "ops": the same CUDA kernels launched one C-ABI call at a time from this module (kept as the readable statement of
         the op sequence and as a cross-check — results are bit-identical).  Both need the library and a GPU; neither does any
-        math in PyTorch."""
+        math in PyTorch.
+
+        Capacities: max_batch pages per encoder call and tables whose K/V cross_kv() holds; s_max self-attention positions
+        (default max_boxes + 72 for tables, + 8 for layout); max_rows decoder rows of decode_rows() and max_prefill_tokens prompt
+        tokens per prefill chunk (0: max_batch, the sizes run_loop uses)."""
         self.lib = _lib.load()
         if impl not in ("native", "ops"):
             raise ValueError(impl)
@@ -143,11 +148,15 @@ class LayoutEngine:
             self.cls_w = T(sd_dec["lm_head.weight"])
             self.bbox_w, self.bbox_b = T(sd_dec["bbox_head.weight"]), T(sd_dec["bbox_head.bias"])
         self.inv_freq = (1.0 / (d.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.int64).float() / hd))).to(dev)
-        self.s_max = d.max_boxes + (72 if d.kind == "table" else 8)     # table prompts carry the query + column boxes
+        # table prompts carry the query + column boxes
+        self.s_max = int(s_max) if s_max is not None else d.max_boxes + (72 if d.kind == "table" else 8)
+        self.max_rows = max(int(max_rows), max_batch) if max_rows else max_batch
+        self.max_prefill_tokens = max(int(max_prefill_tokens), self.max_rows)
+        self._row_max_rows, self._row_max_prefill = int(max_rows), int(max_prefill_tokens)
         if impl == "native":
             self._create_native()
         self._cache_batch = 0
-        self.cross_kv: List[Optional[torch.Tensor]] = [None] * d.num_hidden_layers
+        self._ckv: List[Optional[torch.Tensor]] = [None] * d.num_hidden_layers
         self.kcache: List[torch.Tensor] = []
         self.vcache: List[torch.Tensor] = []
         self.n_enc = 0
@@ -195,6 +204,7 @@ class LayoutEngine:
             c.head_n[i] = n
         c.eos, c.pad = d.eos_token_id, d.pad_token_id
         c.max_batch, c.s_max = self.max_batch, self.s_max
+        c.max_rows, c.max_prefill_tokens = self._row_max_rows, self._row_max_prefill
         self._wt = self._weight_table()          # keeps the device tensors alive
         arr = (ctypes.c_void_p * len(self._wt))(*[t.data_ptr() for t in self._wt])
         self._h = ctypes.c_void_p()
@@ -275,7 +285,7 @@ class LayoutEngine:
     def setup_cache(self, batch: int):
         """SuryaADETRDecoderModel._setup_cache (surya/common/adetr/decoder.py): fresh self / cross caches."""
         d = self.cfg.decoder
-        self.cross_kv = [None] * d.num_hidden_layers
+        self._ckv = [None] * d.num_hidden_layers
         if batch != self._cache_batch:
             shape = (batch, d.num_key_value_heads, self.s_max, d.head_dim)
             self.kcache = [torch.zeros(shape, dtype=self.dtype, device=self.device) for _ in range(d.num_hidden_layers)]
@@ -284,7 +294,7 @@ class LayoutEngine:
         self._slot = torch.arange(batch, dtype=torch.int32, device=self.device)
 
     def clear_cache(self):
-        self.cross_kv = [None] * self.cfg.decoder.num_hidden_layers
+        self._ckv = [None] * self.cfg.decoder.num_hidden_layers
 
     def decode_step(self, boxes: torch.Tensor, enc: torch.Tensor, position, caches=None):
         """One q_len = 1 decoder call (SuryaLayoutDecoder.forward, surya/layout/model/decoder.py:95-126).
@@ -308,9 +318,9 @@ class LayoutEngine:
             raw = x
             n = ops.rmsnorm_adetr(x, L["cross_norm"], d.rms_norm_eps)
             q = ops.gemm(n, L["cq_w"])
-            if self.cross_kv[l] is None:      # K/V of the encoder states, computed at the first call and cached
-                self.cross_kv[l] = ops.gemm(enc2d, L["ckv_w"])
-            a = ops.attn_single_query(q, self.cross_kv[l], Lk, nh, nkv, hd, scale)
+            if self._ckv[l] is None:      # K/V of the encoder states, computed at the first call and cached
+                self._ckv[l] = ops.gemm(enc2d, L["ckv_w"])
+            a = ops.attn_single_query(q, self._ckv[l], Lk, nh, nkv, hd, scale)
             cross = ops.gemm(a, L["co_w"], bias=L["co_b"], residual=raw)
             n = ops.rmsnorm_adetr(cross, L["self_norm"], d.rms_norm_eps)
             qkv = ops.gemm(n, L["sqkv_w"])
@@ -410,7 +420,7 @@ class LayoutEngine:
         st = self._loop_state(B, Lk, n_steps)
         st["enc"].copy_(enc)
         enc2d = st["enc"].view(B * Lk, -1)
-        self.cross_kv = [ops.gemm(enc2d, L["ckv_w"], out=st["ckv"][l]) for l, L in enumerate(self.layers)]
+        self._ckv = [ops.gemm(enc2d, L["ckv_w"], out=st["ckv"][l]) for l, L in enumerate(self.layers)]
         prompt = prompt.to(self.device)
         for j in range(q - 1):
             self.decode_step(prompt[:, j].contiguous(), st["enc"], j, caches=st["caches"])
@@ -442,6 +452,62 @@ class LayoutEngine:
                     self._loop_body(st)
         h = st["hist"]
         return h["tok"][:n_steps], h["bbox"][:n_steps], [x[:n_steps] for x in h["heads"]], h["done"][:n_steps]
+
+
+    # ---------------------------------------------------------------------------------------------- table_rec two-pass flow
+    def cross_kv(self, enc: torch.Tensor):
+        """Project and hold the cross-attention K/V of enc [n_tables, Lk, Henc] (n_tables <= max_batch) for decode_rows().
+        run_loop() overwrites them: call cross_kv() again before the next decode_rows()."""
+        if self.impl != "native":
+            raise _lib.SuryaB200Error("cross_kv / decode_rows need the native engine (impl='native')")
+        if self.kind != "table":
+            raise _lib.SuryaB200Error("cross_kv / decode_rows need a table_rec engine")
+        n = enc.shape[0]
+        if n < 1 or n > self.max_batch:
+            raise _lib.SuryaB200Error(f"{n} tables need max_batch >= {n} (engine has {self.max_batch})")
+        enc_c = enc.to(self.device, self.dtype).contiguous()
+        _lib.check(self.lib.sb_layout_cross_kv(self._h, _lib.ptr(enc_c), ctypes.c_int(n), _lib.stream_ptr()), "sb_layout_cross_kv")
+        self._held = enc_c          # the projection is stream-ordered: keep its input alive until the next call
+        return self
+
+    def decode_rows(self, row_table, prompt: torch.Tensor, n_steps: int):
+        """Greedy decode of rows against the K/V held by cross_kv(): row r attends to table row_table[r].  prompt int64
+        [rows, q, 10]: positions 0..q-2 are prefilled in one batched pass, then q's last token and n_steps-1 generated tokens
+        are decoded, stopping early once every row has produced eos / pad.  Returns (tok [n, rows, 10], bbox [n, rows, 6],
+        heads [list of [n, rows, n_k]], done [n, rows]) for the n <= n_steps steps that ran (n >= the step at which the last
+        row became done; n_steps when some row never does)."""
+        rows, q = int(prompt.shape[0]), int(prompt.shape[1])
+        table = [int(t) for t in (row_table.tolist() if torch.is_tensor(row_table) else row_table)]
+        if len(table) != rows:
+            raise _lib.SuryaB200Error(f"row_table has {len(table)} entries for {rows} prompt rows")
+        if rows < 1 or rows > self.max_rows:
+            raise _lib.SuryaB200Error(f"{rows} rows need max_rows >= {rows} (engine has {self.max_rows})")
+        if q < 1 or n_steps < 1 or q - 1 + n_steps > self.s_max:
+            raise _lib.SuryaB200Error(f"a {q}-token prompt and {n_steps} steps need s_max >= {q - 1 + n_steps} (engine has {self.s_max})")
+        if q - 1 > self.max_prefill_tokens:
+            raise _lib.SuryaB200Error(f"a {q}-token prompt needs max_prefill_tokens >= {q - 1} (engine has {self.max_prefill_tokens})")
+        if self.impl != "native" or self.kind != "table":
+            raise _lib.SuryaB200Error("decode_rows needs a native table_rec engine")
+        d = self.cfg.decoder
+        hk = (rows, n_steps)
+        hist = getattr(self, "_rhist", None)
+        if hist is None or hist["key"] != hk:       # persistent: same pointers -> the step graphs are reused
+            dev, ncol = self.device, d.token_width
+            hist = {"key": hk, "tok": torch.zeros((n_steps, rows, ncol), dtype=torch.int64, device=dev),
+                    "bbox": torch.zeros((n_steps, rows, 6), dtype=torch.float32, device=dev),
+                    "heads": [torch.zeros((n_steps, rows, n), dtype=torch.float32, device=dev) for n in self._head_n],
+                    "done": torch.zeros((n_steps, rows), dtype=torch.uint8, device=dev)}
+            self._rhist = hist
+        prompt_d = prompt.to(self.device, torch.int64).contiguous()
+        tab = (ctypes.c_int * rows)(*table)
+        hp = (ctypes.c_void_p * 4)(*([t.data_ptr() for t in hist["heads"]] + [None] * (4 - len(hist["heads"]))))
+        n_run = ctypes.c_int(0)
+        _lib.check(self.lib.sb_layout_decode_rows(self._h, tab, ctypes.c_int(rows), _lib.ptr(prompt_d), ctypes.c_int(q),
+                                                  ctypes.c_int(n_steps), _lib.ptr(hist["tok"]), _lib.ptr(hist["bbox"]), hp,
+                                                  _lib.ptr(hist["done"]), ctypes.byref(n_run), _lib.stream_ptr()),
+                   "sb_layout_decode_rows")
+        n = n_run.value
+        return hist["tok"][:n], hist["bbox"][:n], [h[:n] for h in hist["heads"]], hist["done"][:n]
 
 
 class _Ns:

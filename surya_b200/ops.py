@@ -409,9 +409,10 @@ def bbox_embed_sum(boxes, tables, hidden, bbox_size, dtype):
     return out
 
 
-def attn_single_query(q, kv, n_keys, nh, nkv, hd, scale, out=None):
-    """q [B, nh*hd]; kv [B*n_keys, 2*nkv*hd] = per token (K heads | V heads), i.e. the fused cross K/V projection output.
-    out: optional row-major [B, nh*hd] view (e.g. a column window of a wider buffer)."""
+def attn_single_query(q, kv, n_keys, nh, nkv, hd, scale, out=None, kv_index=None):
+    """q [B, nh*hd]; kv [S*n_keys, 2*nkv*hd] = per token (K heads | V heads), i.e. the fused cross K/V projection output of S
+    K/V sets (S = B without an index).  out: optional row-major [B, nh*hd] view (e.g. a column window of a wider buffer).
+    kv_index: optional int32 device tensor [B]: query row b reads K/V set kv_index[b] (entries must be in [0, S))."""
     lib = _lib.load()
     B = q.shape[0]
     if out is None:
@@ -420,10 +421,21 @@ def attn_single_query(q, kv, n_keys, nh, nkv, hd, scale, out=None):
     esz = kv.element_size()
     kptr = kv.data_ptr()
     vptr = kptr + nkv * hd * esz
-    check(lib.sb_attn_single_query(dt_code(q.dtype), ptr(q), c_int(_rowmajor(q)), _lib.c_void_p(kptr), _lib.c_void_p(vptr),
-                                   ctypes.c_longlong(n_keys * row), ctypes.c_longlong(hd), ctypes.c_longlong(row), ptr(out),
-                                   c_int(_rowmajor(out)), c_int(B), c_int(nh), c_int(nkv), c_int(hd), c_int(n_keys), c_float(scale),
-                                   stream_ptr()), "sb_attn_single_query")
+    if kv_index is None:
+        check(lib.sb_attn_single_query(dt_code(q.dtype), ptr(q), c_int(_rowmajor(q)), _lib.c_void_p(kptr), _lib.c_void_p(vptr),
+                                       ctypes.c_longlong(n_keys * row), ctypes.c_longlong(hd), ctypes.c_longlong(row), ptr(out),
+                                       c_int(_rowmajor(out)), c_int(B), c_int(nh), c_int(nkv), c_int(hd), c_int(n_keys),
+                                       c_float(scale), stream_ptr()), "sb_attn_single_query")
+        return out
+    n_sets = kv.shape[0] // n_keys
+    if kv_index.dtype != torch.int32 or not kv_index.is_cuda or kv_index.numel() != B:
+        raise _lib.SuryaB200Error("kv_index must be an int32 device tensor with one entry per query row")
+    if B and (int(kv_index.min()) < 0 or int(kv_index.max()) >= n_sets):
+        raise _lib.SuryaB200Error(f"kv_index entries must lie in [0, {n_sets})")
+    check(lib.sb_attn_single_query_rows(dt_code(q.dtype), ptr(q), c_int(_rowmajor(q)), _lib.c_void_p(kptr), _lib.c_void_p(vptr),
+                                        ctypes.c_longlong(n_keys * row), ctypes.c_longlong(hd), ctypes.c_longlong(row), ptr(out),
+                                        c_int(_rowmajor(out)), c_int(B), c_int(nh), c_int(nkv), c_int(hd), c_int(n_keys),
+                                        c_float(scale), ptr(kv_index.contiguous()), stream_ptr()), "sb_attn_single_query_rows")
     return out
 
 
