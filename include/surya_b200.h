@@ -452,8 +452,15 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
 /* table_rec two-pass flow (TableRecPredictor.batch_table_recognition, surya/table_rec/__init__.py:134-236).
  * sb_layout_cross_kv projects the cross-attention K/V of every decoder layer for n_tables <= max_batch encoder states
  * enc [n_tables, Lk, enc_hidden] and holds them.  sb_layout_decode writes the same buffers: after it runs, the held K/V are
- * gone and sb_layout_decode_rows fails until sb_layout_cross_kv is called again. */
+ * gone and sb_layout_decode_rows / sb_layout_step fail until sb_layout_cross_kv is called again. */
 int sb_layout_cross_kv(sb_layout_engine* e, const void* enc, int n_tables, void* stream);
+/* One q_len = 1 decoder call, `model.decoder` in the predictors (surya/layout/model/decoder.py:95-126,
+ * surya/table_rec/model/decoder.py:121-155), either kind.  tok [batch, ncol] int64 and pos [batch] int32 (device): row b
+ * embeds tok[b] at position pos[b] of self-attention cache row b and attends to cross K/V set b of sb_layout_cross_kv, with
+ * 1 <= batch <= n_tables.  Outputs (device, f32): bbox [batch, 6] (sigmoid), heads[k] [batch, head_n[k]].  Runs on `stream`
+ * without a graph; pos[b] must be below s_max. */
+int sb_layout_step(sb_layout_engine* e, const long long* tok, const int* pos, int batch, float* bbox, float* const* heads,
+                   void* stream);
 /* Greedy decode of `rows` (<= max_rows) sequences against the held K/V: row r attends to table row_table_host[r] (HOST
  * int32 [rows], each in [0, n_tables)).  prompt [rows, q_len, ncol] int64 (device): positions 0 .. q_len-2 go through the
  * decoder as one batched prefill (rows * (q_len-1) GEMM rows, in chunks of at most max(max_rows, max_prefill_tokens) tokens),

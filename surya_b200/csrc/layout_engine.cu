@@ -1,9 +1,9 @@
 // surya_b200 — layout / table_rec engine: Donut-Swin encoder + ADETR box decoder behind the C ABI (sb_layout_*).
 //
-// Same kernels and the same op order as the op-by-op path in surya_b200/layout.py (impl="ops": one C-ABI call per kernel; it stays as the readable
-// statement of the sequence and as a cross-check: tests require bit-identical results); here the layer loops, the
-// workspaces, the K/V caches and the greedy decode loop (one CUDA graph per 8 steps) live in C++ so that nothing on the
-// forward path depends on the host between the first and the last kernel.
+// The layer loops, the workspaces, the K/V caches and the greedy decode loop (one CUDA graph per 8 steps) live here so that
+// nothing on the forward path depends on the host between the first and the last kernel.  Every decoder call, the greedy
+// loop's steps, the predictors' single steps (sb_layout_step) and the table cell pass, goes through run_token: one statement of
+// the decoder's op order.
 //
 // Reference: DonutSwinLayoutModel.forward / DonutSwinModel.forward (surya/layout/model/encoder.py:33-81,
 // surya/table_rec/model/encoder.py:35-87), DonutSwinEncoder/Stage/Layer (surya/common/donut/encoder.py:534-931),
@@ -400,6 +400,30 @@ int sb_layout_cross_kv(sb_layout_engine* e, const void* enc, int n_tables, void*
                                c.enc_hidden, nullptr), st));
   e->held_gen = ++e->kv_gen;
   e->held_tables = n_tables;
+  return 0;
+}
+
+int sb_layout_step(sb_layout_engine* e, const long long* tok, const int* pos, int batch, float* bbox, float* const* heads,
+                   void* stream) {
+  if (!e || !tok || !pos || !bbox || !heads) { set_error("sb_layout_step: null argument"); return -1; }
+  const sb_layout_config& c = e->c;
+  for (int k = 0; k < c.n_out_heads; ++k)
+    if (!heads[k]) { set_error("sb_layout_step: head output %d is null", k); return -1; }
+  if (e->held_gen == 0 || e->held_gen != e->kv_gen) {
+    set_error("sb_layout_step: no cross K/V held (sb_layout_decode overwrote them, or sb_layout_cross_kv was not called)");
+    return -3;
+  }
+  if (batch <= 0 || batch > e->held_tables) {
+    set_error("sb_layout_step: batch %d outside 1..%d (the tables held by sb_layout_cross_kv)", batch, e->held_tables);
+    return -2;
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CK(run_token(e, tok, pos, batch, st));
+  const size_t B = static_cast<size_t>(batch);
+  bool ok = cudaMemcpyAsync(bbox, e->out_bbox, B * 6 * sizeof(float), cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+  for (int k = 0; k < c.n_out_heads && ok; ++k)
+    ok = cudaMemcpyAsync(heads[k], e->out_head[k], B * c.head_n[k] * sizeof(float), cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+  if (!ok) { cudaGetLastError(); set_error("sb_layout_step: output copy failed"); return -5; }
   return 0;
 }
 

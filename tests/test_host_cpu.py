@@ -281,12 +281,12 @@ def test_table_oracle_pinned_to_reference_golden():
     assert torch.equal(tok, g["tokens"])
 
 
-def test_layout_weight_table_matches_the_c_abi_layout():
-    """LayoutEngine._weight_table order / count vs the SB_LW_* layout in include/surya_b200.h (what sb_layout_create checks)."""
+def test_packed_layout_weights_match_the_c_abi_layout():
+    """pack_layout_weights order / count vs the SB_LW_* layout in include/surya_b200.h (what sb_layout_create checks)."""
     import re
 
     from surya_b200.config import layout_tiny, table_tiny
-    from surya_b200.layout import LayoutEngine
+    from surya_b200.layout import pack_layout_weights
     from surya_b200.synth import adetr_layout_state_dict, adetr_table_state_dict, swin_state_dict
 
     hdr = (ROOT / "include" / "surya_b200.h").read_text()
@@ -297,15 +297,7 @@ def test_layout_weight_table_matches_the_c_abi_layout():
     n_fixed, n_layer, n_dec, n_tail = enum_size("SB_LW_ENC_FIXED"), enum_size("SB_LW_ENC_LAYER"), enum_size("SB_LW_DEC_LAYER"), enum_size("SB_LW_DEC_TAIL")
     assert (n_fixed, n_layer, n_dec, n_tail) == (5, 13, 12, 4)
     for cfg, sdd, tables, heads in ((layout_tiny(), adetr_layout_state_dict, 15, 3), (table_tiny(), adetr_table_state_dict, 13, 5)):
-        eng = LayoutEngine.__new__(LayoutEngine)          # pack on the CPU without creating the CUDA engine
-        import surya_b200.layout as LM
-        orig = LM._lib.load
-        LM._lib.load = lambda *a, **k: None
-        try:
-            LayoutEngine.__init__(eng, cfg, swin_state_dict(cfg.encoder, 0), sdd(cfg.decoder, 0), device="cpu", impl="ops")
-        finally:
-            LM._lib.load = orig
-        w = eng._weight_table()
+        w = pack_layout_weights(cfg, swin_state_dict(cfg.encoder, 0), sdd(cfg.decoder, 0), torch.float16, device="cpu")
         e, d = cfg.encoder, cfg.decoder
         want = n_fixed + sum(1 + dep * n_layer for dep in e.depths) + 3 * (len(e.depths) - 1) + tables + d.num_hidden_layers * n_dec + n_tail + heads
         assert len(w) == want

@@ -223,10 +223,9 @@ def test_swin_encoder_vs_reference_golden(built_lib, dtype, tol):
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float16, 1e-2), (torch.bfloat16, 6e-2)])
-def test_swin_encoder_window_padding_vs_reference_golden(built_lib, dtype, tol):
+def test_engine_swin_encoder_window_padding_vs_reference_golden(built_lib, dtype, tol):
     """288x352 input: token grids 36x44, 18x22 and 9x11 are not multiples of the 8x8 window, so the reference pads them
-    (donut/encoder.py:591-596).  Engine (C++ loop) and the op-by-op path vs the reference's own output, and bit-identical to each
-    other."""
+    (donut/encoder.py:591-596).  Engine vs the reference's own output."""
     from surya_b200.config import LayoutConfig, SwinConfig, table_decoder
     from surya_b200.layout import LayoutEngine
     from surya_b200.synth import adetr_table_state_dict, layout_synthetic_pages, swin_state_dict
@@ -238,18 +237,14 @@ def test_swin_encoder_window_padding_vs_reference_golden(built_lib, dtype, tol):
     x = layout_synthetic_pages(1, enc_cfg.image_size, seed=g["meta"]["page_seed"])
     assert abs(float(x.double().sum()) - float(g["input_checksum"])) < 1e-6
     ref = g["encoder"]
-    outs = []
-    for impl in ("native", "ops"):
-        eng = LayoutEngine(cfg, sde, sdd, dtype=dtype, impl=impl)
-        enc = eng.encode(x.cuda())
-        outs.append(enc)
-        encf = enc.float().cpu()
-        err = (encf - ref).abs().max().item()
-        rel = ((encf - ref).norm() / ref.norm()).item()
-        print(f"swin encoder with window padding, {impl}, {dtype}: max abs err {err:.4g} (ref max {ref.abs().max():.3g}), rel fro {rel:.3g}")
-        assert enc.shape == (1, 99, 1024)
-        assert err < tol * ref.abs().max().item() and rel < tol / 4
-    assert torch.equal(outs[0], outs[1])
+    eng = LayoutEngine(cfg, sde, sdd, dtype=dtype)
+    enc = eng.encode(x.cuda())
+    encf = enc.float().cpu()
+    err = (encf - ref).abs().max().item()
+    rel = ((encf - ref).norm() / ref.norm()).item()
+    print(f"swin encoder with window padding, {dtype}: max abs err {err:.4g} (ref max {ref.abs().max():.3g}), rel fro {rel:.3g}")
+    assert enc.shape == (1, 99, 1024)
+    assert err < tol * ref.abs().max().item() and rel < tol / 4
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float16, 1e-2), (torch.bfloat16, 6e-2)])
@@ -564,10 +559,16 @@ def test_graph_replayed_loop_equals_eager_loop(built_lib, kind):
 
 
 @pytest.mark.parametrize("kind", ["layout", "table"])
-def test_native_engine_equals_op_by_op_path(built_lib, kind):
-    """sb_layout_encode / sb_layout_decode (layer loops, caches and the decode loop in C++) vs the same kernels launched op by
-    op from Python: encoder states, tokens and head outputs must be bit-identical, with and without graphs."""
-    from surya_b200.layout import LayoutEngine
+def test_model_surface_steps_equal_the_graph_loop(built_lib, kind):
+    """decode_prompt / decode_step (sb_layout_step, one C call per step) vs run_loop (sb_layout_decode, steps replayed as
+    graphs): fed the same prompt and then the loop's own tokens, every step's bbox and head outputs are bit-identical, since
+    both run the same decoder call on the same row count.  Also: the loop's histories with and without graphs, the encoder's
+    max_batch chunking, and the refusals of the step entry."""
+    import ctypes
+
+    from surya_b200 import _lib
+    from surya_b200.layout import LayoutEngine, _head_ptrs
+    from surya_b200.synth import TABLE_HEADS
 
     if kind == "layout":
         cfg, g, sde, sdd, x = _tiny()
@@ -575,22 +576,52 @@ def test_native_engine_equals_op_by_op_path(built_lib, kind):
     else:
         cfg, g, sde, sdd, x, prompt = _table_tiny()
         prompt = prompt.cuda()
-    nat = LayoutEngine(cfg, sde, sdd, dtype=torch.float16, impl="native", max_batch=4)
-    ref = LayoutEngine(cfg, sde, sdd, dtype=torch.float16, impl="ops")
-    assert nat.workspace_bytes > 0
+    eng = LayoutEngine(cfg, sde, sdd, dtype=torch.float16, max_batch=4)
+    assert eng.workspace_bytes > 0
     x = x.cuda()
-    enc_n, enc_p = nat.encode(x), ref.encode(x)
-    assert torch.equal(enc_n, enc_p)
+    enc = eng.encode(x)
     # batch larger than max_batch is cut into chunks by the binding
     x6 = torch.cat([x, x, x], 0)
-    assert torch.equal(nat.encode(x6), torch.cat([enc_n, enc_n, enc_n], 0))
-    steps = 11
-    want = [t.clone() for t in _flatten(ref.run_loop(enc_p, prompt, steps, use_graph=False))]
-    for use_graph in (False, True, True):
-        got = _flatten(nat.run_loop(enc_n, prompt, steps, use_graph=use_graph))
+    assert torch.equal(eng.encode(x6), torch.cat([enc, enc, enc], 0))
+    steps, q = 11, prompt.shape[1]
+    want = [t.clone() for t in _flatten(eng.run_loop(enc, prompt, steps, use_graph=False))]
+    for use_graph in (True, True):
+        got = _flatten(eng.run_loop(enc, prompt, steps, use_graph=use_graph))
         for a, b in zip(got, want):
             assert torch.equal(a, b)
-    nat.close()
+    tok, bbox, heads = want[0], want[1], want[2:-1]
+
+    def outputs(out):
+        return [out[k] for k in TABLE_HEADS] if kind == "table" else list(out)
+
+    eng.setup_cache(2)
+    for s in range(steps):
+        out = eng.decode_prompt(prompt, enc, 0) if s == 0 else eng.decode_step(tok[s - 1], enc, q - 1 + s)
+        for a, b in zip(outputs(out), [bbox[s]] + [h[s] for h in heads]):
+            assert torch.equal(a, b), s
+
+    # refusals: a batch above max_batch at the model surface; at the C entry, a batch above the held tables and K/V that
+    # sb_layout_decode has overwritten
+    with pytest.raises(_lib.SuryaB200Error, match="max_batch 4"):
+        eng.setup_cache(5)
+    B = 3
+    t = torch.zeros((B, cfg.decoder.token_width), dtype=torch.int64, device="cuda")
+    p = torch.zeros(B, dtype=torch.int32, device="cuda")
+    bb = torch.empty((B, 6), dtype=torch.float32, device="cuda")
+    hs = [torch.empty((B, n), dtype=torch.float32, device="cuda") for n in eng._head_n]
+
+    def step(n):
+        return eng.lib.sb_layout_step(eng._h, _lib.ptr(t), _lib.ptr(p), ctypes.c_int(n), _lib.ptr(bb), _head_ptrs(hs),
+                                      _lib.stream_ptr())
+
+    assert step(3) != 0                     # two tables held
+    eng.run_loop(enc, prompt, steps)
+    assert step(2) != 0
+    # the loop left the self-attention caches the steps above wrote; decode_step projects the cross K/V again
+    out = eng.decode_step(tok[steps - 2], enc, q - 2 + steps)
+    for a, b in zip(outputs(out), [bbox[steps - 1]] + [h[steps - 1] for h in heads]):
+        assert torch.equal(a, b)
+    eng.close()
 
 
 def _flatten(res):
@@ -598,7 +629,7 @@ def _flatten(res):
     return [tok, bbox] + list(heads) + [done]
 
 
-def test_nonsquare_encoder_and_cellpass_prompt_vs_reference_golden(built_lib):
+def test_engine_nonsquare_encoder_and_cellpass_prompt_vs_reference_golden(built_lib):
     """256x512 input (non-square Swin grid) and a 7-token table_rec cell-pass prompt, both against the second reference
     fixture: encoder states, then the heads of the first generated position after the multi-token prompt."""
     from surya_b200.config import LayoutConfig, SwinConfig, table_decoder
@@ -610,15 +641,14 @@ def test_nonsquare_encoder_and_cellpass_prompt_vs_reference_golden(built_lib):
     cfg = LayoutConfig(encoder=enc_cfg, decoder=table_decoder(2))
     sde, sdd = swin_state_dict(enc_cfg, g["meta"]["seed"]), adetr_table_state_dict(cfg.decoder, g["meta"]["seed"])
     x = layout_synthetic_pages(2, enc_cfg.image_size, seed=g["meta"]["page_seed"])
-    for impl in ("native", "ops"):
-        eng = LayoutEngine(cfg, sde, sdd, dtype=torch.float16, impl=impl, max_batch=2)
-        enc = eng.encode(x.cuda())
-        ref = g["encoder"]
-        rel = ((enc.float().cpu() - ref).norm() / ref.norm()).item()
-        assert enc.shape == ref.shape and rel < 5e-3, (impl, rel)
-        tok, bbox, heads, done = eng.run_loop(ref.to(torch.float16).cuda(), g["prompt"].cuda(), 1, use_graph=False)
-        got = {"bbox": bbox[0], "category": heads[0][0], "merges": heads[1][0], "colspan": heads[2][0], "is_header": heads[3][0]}
-        for k, v in got.items():
-            err = (v.cpu() - g["heads"][k][:, 0]).abs().max().item()
-            assert err < 1e-2 * max(1.0, g["heads"][k].abs().max().item()), (impl, k, err)
-        eng.close()
+    eng = LayoutEngine(cfg, sde, sdd, dtype=torch.float16, max_batch=2)
+    enc = eng.encode(x.cuda())
+    ref = g["encoder"]
+    rel = ((enc.float().cpu() - ref).norm() / ref.norm()).item()
+    assert enc.shape == ref.shape and rel < 5e-3, rel
+    tok, bbox, heads, done = eng.run_loop(ref.to(torch.float16).cuda(), g["prompt"].cuda(), 1, use_graph=False)
+    got = {"bbox": bbox[0], "category": heads[0][0], "merges": heads[1][0], "colspan": heads[2][0], "is_header": heads[3][0]}
+    for k, v in got.items():
+        err = (v.cpu() - g["heads"][k][:, 0]).abs().max().item()
+        assert err < 1e-2 * max(1.0, g["heads"][k].abs().max().item()), (k, err)
+    eng.close()

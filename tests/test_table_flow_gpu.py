@@ -98,7 +98,7 @@ def test_early_exit_stops_before_the_budget(built_lib):
 
 def test_batched_prefill_vs_reference_cellpass_golden(built_lib):
     """7-token cell prompt prefilled in one pass (rows x 6 GEMM rows) against the reference's batched prefill, within the
-    tolerances test_nonsquare_encoder_and_cellpass_prompt_vs_reference_golden uses for the position-by-position path."""
+    tolerances test_engine_nonsquare_encoder_and_cellpass_prompt_vs_reference_golden uses for the position-by-position path."""
     from surya_b200.config import LayoutConfig, SwinConfig, table_decoder
     from surya_b200.layout import LayoutEngine
     from surya_b200.synth import adetr_table_state_dict, swin_state_dict
