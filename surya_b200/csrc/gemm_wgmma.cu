@@ -17,6 +17,10 @@
 // only the single-pass 16-bit staged epilogue, no grouped mode and no fallback epilogue (epilogue_chunk, a __noinline__
 // call).  Without them ptxas gives it no stack frame and, at BN = 128, no spills, and the decode GEMMs run faster
 // (DESIGN.md §5).  Both variants give the same bits.
+//
+// STAGED = true is the plain variant for launches the 16-bit staged epilogue takes (epilogue_v2_ok) outside grouped mode: the
+// same code with the fallback epilogue and the grouped A offset compiled out, as in the decode variant.  At BN = 128 that
+// removes the plain variant's stack frame and spills.  Same bits: it runs the staged epilogue the plain variant would.
 #include "gemm.cuh"
 
 #include <string>
@@ -41,7 +45,7 @@ __device__ __forceinline__ void tile_coords(int tile, int m_blocks, int n_blocks
   nb = r / gsz;
 }
 
-template <typename T, int BN, int STAGES, bool DECODE>
+template <typename T, int BN, int STAGES, bool DECODE, bool STAGED = false>
 __global__ void __launch_bounds__(384, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                const GemmKParams p) {
@@ -49,6 +53,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int AC = acc_cols<BN>();
   static_assert(!DECODE || BN <= ACC_MAX_COLS, "the decode variant takes single-pass epilogue tiles only");
+  static_assert(!STAGED || (!DECODE && BN <= ACC_MAX_COLS), "the staged plain variant takes single-pass epilogue tiles only");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // array + offset keeps the shared address space (STS / LDS, not generic ST / LD)
@@ -109,11 +114,11 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           // before its B tile, the decode variant after it: one order for both was slower on H100 for prefill or for the
           // decode step, whichever it did not come from (DESIGN.md §5).  Grouped mode: A columns of this n-block's group.
           const bool b_in_flight = tile == static_cast<int>(blockIdx.x) && kb < early;
-          if (!DECODE && b_in_flight) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + nb * p.group_k, mb * BM);
+          if (!DECODE && b_in_flight) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + (STAGED ? 0 : nb * p.group_k), mb * BM);
           if (!b_in_flight) {
             mbar_wait(&empty_bar[s], ph ^ 1);
             mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-            if (!DECODE) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + nb * p.group_k, mb * BM);
+            if (!DECODE) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK + (STAGED ? 0 : nb * p.group_k), mb * BM);
             tma_load_2d(sbp, &tma_b, &full_bar[s], kb * BK, nb * BN);
           }
           if (DECODE) tma_load_2d(sa, &tma_a, &full_bar[s], kb * BK, mb * BM);
@@ -134,7 +139,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     int s = 0;
     uint32_t ph = 0;
     const bool vec_ok = (p.ldc % 8 == 0) && (!p.residual || p.ldr % 8 == 0);
-    const bool v2 = DECODE || epilogue_v2_ok(p);   // the host refuses decode launches the staged epilogue cannot take
+    const bool v2 = DECODE || STAGED || epilogue_v2_ok(p);   // the host launches these variants only where it applies
     const AccRow acc(acc_s, q * 32 + lane, AC);
     float d[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -323,12 +328,12 @@ template <int BN, int STAGES> constexpr size_t gemm_smem_bytes() {
   return STAGES * (128 * 64 * 2 + BN * 64 * 2) + 1024 /*align slack*/ + 256 /*barriers*/ + acc_smem_bytes<BN>() + epi_smem_bytes<BN>();
 }
 
-template <typename T, int BN, int STAGES, bool DECODE>
+template <typename T, int BN, int STAGES, bool DECODE, bool STAGED = false>
 static int launch_cfg(const GemmArgs& a, cudaStream_t stream) {
   constexpr size_t SMEM = gemm_smem_bytes<BN, STAGES>();
   static_assert(SMEM <= SMEM_LIMIT, "GEMM tile does not fit in shared memory");
   static bool attr_set = false;
-  auto kern = gemm_tn_kernel<T, BN, STAGES, DECODE>;
+  auto kern = gemm_tn_kernel<T, BN, STAGES, DECODE, STAGED>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
     if (e != cudaSuccess) {
@@ -355,7 +360,11 @@ static int launch_cfg(const GemmArgs& a, cudaStream_t stream) {
 template <typename T, bool DECODE>
 static int launch_bn(const GemmArgs& a, int bn, cudaStream_t stream) {
   switch (bn) {
-    case 128: return launch_cfg<T, 128, 4, DECODE>(a, stream);
+    case 128:
+      // plain launches the staged epilogue takes run without the fallback epilogue (BN 128 only: the width where it costs
+      // the plain variant spills)
+      if (!DECODE && !a.group_k && epilogue_v2_ok(gemm_kparams(a))) return launch_cfg<T, 128, 4, false, true>(a, stream);
+      return launch_cfg<T, 128, 4, DECODE>(a, stream);
     case 64: return launch_cfg<T, 64, 6, DECODE>(a, stream);
     case 32: return launch_cfg<T, 32, 8, DECODE>(a, stream);
   }
