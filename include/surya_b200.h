@@ -283,6 +283,29 @@ int sb_det_normalize_u8(int dtype, const unsigned char* pages_nhwc, void* out_nc
 int sb_det_text_front(int dtype, const void* logits, int n_labels, int B, int hs, int ws, int HO, int WO, void* map16,
                       unsigned char* mask, float* thresholds, unsigned int* hist_scratch, float text_threshold, float low_text,
                       void* stream);
+/* Pages of any size (replaces DetectionPredictor's host PIL chain: surya/detection/util.py:7-36 split_image + ImageOps.pad,
+ * surya/detection/__init__.py:50-62 prepare_image = thumbnail(LANCZOS, reducing_gap=2.0) + resize(LANCZOS)):
+ * ragged uint8 HWC pages packed back to back in `pages` -> processor-size uint8 HWC chunks in `out`, byte-equal to PIL.
+ * surya_b200/page_prep.py plans each chunk as a chain of jobs, one per step (n_steps launches, step s runs step_jobs[s]
+ * jobs, the largest writing step_max_px[s] pixels; step_jobs / step_max_px are host arrays), each job an int64 row of 16:
+ *   kind (0 box-average reduce by fx x fy, 1 horizontal / 2 vertical Lanczos pass), source byte offset, source w, h,
+ *   source rows before the padding rows (read as ImageOps.pad's (255, 0, 0)), source in pages (1) or scratch (0),
+ *   destination byte offset, destination w, h, destination in out (1) or scratch (0), fx, fy, taps per output pixel,
+ *   weight offset and bounds offset (int32 elements of `tables`: PIL's 22-bit fixed-point weights [n_out, taps] and
+ *   (first tap, tap count) [n_out, 2]).
+ * scratch holds the intermediate images of the chains (byte size from the planner; may be null when no job uses it). */
+int sb_det_page_resize(const unsigned char* pages, unsigned char* scratch, unsigned char* out, const long long* jobs,
+                       const int* tables, int n_steps, const int* step_jobs, const long long* step_max_px, void* stream);
+/* sb_det_text_front over chunks of tall pages, stitched like DetectionPredictor.batch_detection (surya/detection/__init__.py:
+ * 134-151): chunk c (logits [n_chunks, n_labels, hs, ws]) is up-sampled to HO x WO and its first chunk_tab[c][2] rows are written
+ * at row chunk_tab[c][1] of the packed map16 [sum of page rows, WO]; chunk_tab int32 [n_chunks, 4] = page, row, rows kept, 0.
+ * The dynamic thresholds come from one histogram over the whole stitched page (get_dynamic_thresholds over the stacked heatmap)
+ * and the mask is map > low_text(page).  page_tab int32 [n_pages, 2] = first row, rows of each page; max_page_rows its largest
+ * rows; thresholds [n_pages, 4]; hist_scratch [n_pages, 16384] uint32, zero on entry, zero on exit. */
+int sb_det_text_front_stitched(int dtype, const void* logits, int n_labels, int n_chunks, int hs, int ws, int HO, int WO,
+                               const int* chunk_tab, int n_pages, const int* page_tab, int max_page_rows, void* map16,
+                               unsigned char* mask, float* thresholds, unsigned int* hist_scratch, float text_threshold,
+                               float low_text, void* stream);
 /* Back half of the detection post-processing on the device (surya/detection/heatmap.py:33-107, detect_boxes after the mask),
  * fed by sb_det_text_front's map16 [B,H,W] (dtype fp16 / bf16), mask [B,H,W] uint8 and thresholds [B,4]:
  * cv2.connectedComponentsWithStats(connectivity=4) (components numbered in raster order of their first pixel), the

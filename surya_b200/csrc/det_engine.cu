@@ -190,6 +190,28 @@ int sb_det_text_front(int dtype, const void* logits, int n_labels, int B, int hs
                         low_text, static_cast<cudaStream_t>(stream));
 }
 
+int sb_det_text_front_stitched(int dtype, const void* logits, int n_labels, int n_chunks, int hs, int ws, int HO, int WO,
+                               const int* chunk_tab, int n_pages, const int* page_tab, int max_page_rows, void* map16,
+                               unsigned char* mask, float* thresholds, unsigned int* hist_scratch, float text_threshold,
+                               float low_text, void* stream) {
+  if (!logits || !chunk_tab || !page_tab || !map16 || !mask || !thresholds || !hist_scratch) {
+    set_error("sb_det_text_front_stitched: null argument");
+    return -1;
+  }
+  if (n_chunks < 0 || n_pages < 0 || max_page_rows < 0) { set_error("sb_det_text_front_stitched: negative count"); return -1; }
+  return det_text_front(dtype, logits, n_labels, n_chunks, hs, ws, HO, WO, map16, mask, thresholds, hist_scratch, text_threshold,
+                        low_text, static_cast<cudaStream_t>(stream), chunk_tab, n_pages, page_tab, max_page_rows);
+}
+
+int sb_det_page_resize(const unsigned char* pages, unsigned char* scratch, unsigned char* out, const long long* jobs,
+                       const int* tables, int n_steps, const int* step_jobs, const long long* step_max_px, void* stream) {
+  if (!pages || !out || !jobs || !tables || (n_steps > 0 && (!step_jobs || !step_max_px))) {
+    set_error("sb_det_page_resize: null argument");
+    return -1;
+  }
+  return det_page_resize(pages, scratch, out, jobs, tables, n_steps, step_jobs, step_max_px, static_cast<cudaStream_t>(stream));
+}
+
 int sb_det_text_boxes(int dtype, const void* map16, const unsigned char* mask, const float* thresholds, int B, int H, int W,
                       int max_boxes, int max_points, void* scratch, size_t scratch_bytes, int* count, int* overflow, int* box,
                       float* peak, int* points, void* stream) {

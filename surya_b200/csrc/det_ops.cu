@@ -591,27 +591,32 @@ __device__ __forceinline__ unsigned short bits16(float v) {
   return *reinterpret_cast<unsigned short*>(&t);
 }
 
+// chunk_tab (optional, int32 [n_chunks, 4]): chunk c = blockIdx.y belongs to page chunk_tab[c][0] and writes its first
+// chunk_tab[c][2] rows at row chunk_tab[c][1] of the packed stitched map; without it chunk c is page c at row c * HO.
 template <typename T>
 __global__ void __launch_bounds__(256) det_front_map_kernel(const T* __restrict__ logits, int plane_stride, T* __restrict__ map,
                                                             unsigned int* __restrict__ hist, int hs, int ws, int HO, int WO,
-                                                            int rows_per_block) {
-  // block = rows_per_block output rows of page blockIdx.y; thread = 4 consecutive columns at a time
+                                                            int rows_per_block, const int* __restrict__ chunk_tab) {
+  // block = rows_per_block output rows of chunk blockIdx.y; thread = 4 consecutive columns at a time
   extern __shared__ unsigned int sh[];
   for (int i = threadIdx.x; i < FRONT_BINS; i += 256) sh[i] = 0u;
   __syncthreads();
-  const int pg = blockIdx.y;
-  const T* in = logits + static_cast<size_t>(pg) * plane_stride;
+  const int ch = blockIdx.y;
+  const int pg = chunk_tab ? chunk_tab[ch * 4 + 0] : ch;
+  const int row0 = chunk_tab ? chunk_tab[ch * 4 + 1] : ch * HO;
+  const int rows = chunk_tab ? chunk_tab[ch * 4 + 2] : HO;
+  const T* in = logits + static_cast<size_t>(ch) * plane_stride;
   const int oy0 = blockIdx.x * rows_per_block;
   for (int r = 0; r < rows_per_block; ++r) {
     const int oy = oy0 + r;
-    if (oy >= HO) break;
+    if (oy >= rows) break;
     const float sy = fmaxf((oy + 0.5f) * (static_cast<float>(hs) / HO) - 0.5f, 0.f);
     const int y0 = static_cast<int>(sy);
     const int y1 = y0 + (y0 < hs - 1 ? 1 : 0);
     const float ly = sy - y0, hy = 1.f - ly;
     const T* r0 = in + static_cast<size_t>(y0) * ws;
     const T* r1 = in + static_cast<size_t>(y1) * ws;
-    T* orow = map + (static_cast<size_t>(pg) * HO + oy) * WO;
+    T* orow = map + (static_cast<size_t>(row0) + oy) * WO;
     for (int ox = threadIdx.x; ox < WO; ox += 256) {
       const float sx = fmaxf((ox + 0.5f) * (static_cast<float>(ws) / WO) - 0.5f, 0.f);
       const int x0 = static_cast<int>(sx);
@@ -632,15 +637,18 @@ __global__ void __launch_bounds__(256) det_front_map_kernel(const T* __restrict_
     if (sh[i]) atomicAdd(&gh[i], sh[i]);
 }
 
+// page_tab (optional, int32 [B, 2]): page b spans page_tab[b][1] rows of WO pixels from row page_tab[b][0] of the packed map;
+// without it every page has n_pix pixels from pixel b * n_pix.
 template <typename T>
 __global__ void __launch_bounds__(256) det_front_threshold_kernel(unsigned int* __restrict__ hist, float* __restrict__ thr,
                                                                   long long n_pix, float text_threshold, float low_text,
-                                                                  float typical) {
+                                                                  float typical, const int* __restrict__ page_tab, int WO) {
   // one block per page: walk the histogram from the top bin down until n - int(0.9 n) pixels are covered
   __shared__ unsigned int cnt[256];
   __shared__ double sum[256];
   __shared__ long long s_before[257];
   unsigned int* gh = hist + static_cast<size_t>(blockIdx.x) * FRONT_BINS;
+  if (page_tab) n_pix = static_cast<long long>(page_tab[blockIdx.x * 2 + 1]) * WO;
   const long long k = n_pix - static_cast<long long>(static_cast<double>(n_pix) * 0.9);   // int(len * 0.9) truncates
   constexpr int PER = FRONT_BINS / 256;
   // thread t owns bins [hi - PER + 1, hi] counted from the top: t = 0 holds the largest values
@@ -691,10 +699,16 @@ __global__ void __launch_bounds__(256) det_front_threshold_kernel(unsigned int* 
 
 template <typename T>
 __global__ void __launch_bounds__(256) det_front_mask_kernel(const T* __restrict__ map, const float* __restrict__ thr,
-                                                             unsigned char* __restrict__ mask, long long n_pix) {
+                                                             unsigned char* __restrict__ mask, long long n_pix,
+                                                             const int* __restrict__ page_tab, int WO) {
   const float low = thr[blockIdx.y * 4 + 1];
-  const T* m = map + static_cast<size_t>(blockIdx.y) * n_pix;
-  unsigned char* o = mask + static_cast<size_t>(blockIdx.y) * n_pix;
+  size_t base = static_cast<size_t>(blockIdx.y) * n_pix;
+  if (page_tab) {
+    base = static_cast<size_t>(page_tab[blockIdx.y * 2]) * WO;
+    n_pix = static_cast<long long>(page_tab[blockIdx.y * 2 + 1]) * WO;
+  }
+  const T* m = map + base;
+  unsigned char* o = mask + base;
   const long long i0 = (static_cast<long long>(blockIdx.x) * 256 + threadIdx.x) * 8;
   if (i0 + 8 <= n_pix) {
     const uint4 u = *reinterpret_cast<const uint4*>(m + i0);
@@ -709,32 +723,36 @@ __global__ void __launch_bounds__(256) det_front_mask_kernel(const T* __restrict
 }
 
 int det_text_front(int dtype, const void* logits, int n_labels, int B, int hs, int ws, int HO, int WO, void* map16,
-                   unsigned char* mask, float* thr, unsigned int* hist, float text_threshold, float low_text, cudaStream_t st) {
+                   unsigned char* mask, float* thr, unsigned int* hist, float text_threshold, float low_text, cudaStream_t st,
+                   const int* chunk_tab, int n_pages, const int* page_tab, int max_page_rows) {
   if (B <= 0) return 0;
   if (B > 65535) { set_error("det_text_front: too many pages for the grid"); return -1; }
   const long long n_pix = static_cast<long long>(HO) * WO;
-  if (n_pix % 8) { set_error("det_text_front: H*W must be a multiple of 8"); return -1; }
+  if (n_pix % 8 || (chunk_tab && WO % 8)) { set_error("det_text_front: H*W (stitched: W) must be a multiple of 8"); return -1; }
+  if (!chunk_tab) { n_pages = B; max_page_rows = HO; }
+  if (n_pages <= 0) return 0;
+  if (n_pages > 65535) { set_error("det_text_front: too many pages for the grid"); return -1; }
   const int rows_per_block = 16;
   dim3 g1((HO + rows_per_block - 1) / rows_per_block, B);
   const size_t smem = FRONT_BINS * sizeof(unsigned int);
-  const int plane_stride = n_labels * hs * ws;         // channel 0 of page b
-  dim3 g3(static_cast<unsigned int>((n_pix / 8 + 255) / 256), B);
+  const int plane_stride = n_labels * hs * ws;         // channel 0 of chunk b
+  dim3 g3(static_cast<unsigned int>((static_cast<long long>(max_page_rows) * WO / 8 + 255) / 256), n_pages);
   if (dtype == DT_F16) {
     static bool attr = false;
     if (!attr) { cudaFuncSetAttribute(det_front_map_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
-    det_front_map_kernel<__half><<<g1, 256, smem, st>>>((const __half*)logits, plane_stride, (__half*)map16, hist, hs, ws, HO, WO, rows_per_block);
+    det_front_map_kernel<__half><<<g1, 256, smem, st>>>((const __half*)logits, plane_stride, (__half*)map16, hist, hs, ws, HO, WO, rows_per_block, chunk_tab);
     if (int rc = launch_ok()) return rc;
-    det_front_threshold_kernel<__half><<<B, 256, 0, st>>>(hist, thr, n_pix, text_threshold, low_text, 0.7f);
+    det_front_threshold_kernel<__half><<<n_pages, 256, 0, st>>>(hist, thr, n_pix, text_threshold, low_text, 0.7f, page_tab, WO);
     if (int rc = launch_ok()) return rc;
-    det_front_mask_kernel<__half><<<g3, 256, 0, st>>>((const __half*)map16, thr, mask, n_pix);
+    det_front_mask_kernel<__half><<<g3, 256, 0, st>>>((const __half*)map16, thr, mask, n_pix, page_tab, WO);
   } else {
     static bool attr = false;
     if (!attr) { cudaFuncSetAttribute(det_front_map_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
-    det_front_map_kernel<__nv_bfloat16><<<g1, 256, smem, st>>>((const __nv_bfloat16*)logits, plane_stride, (__nv_bfloat16*)map16, hist, hs, ws, HO, WO, rows_per_block);
+    det_front_map_kernel<__nv_bfloat16><<<g1, 256, smem, st>>>((const __nv_bfloat16*)logits, plane_stride, (__nv_bfloat16*)map16, hist, hs, ws, HO, WO, rows_per_block, chunk_tab);
     if (int rc = launch_ok()) return rc;
-    det_front_threshold_kernel<__nv_bfloat16><<<B, 256, 0, st>>>(hist, thr, n_pix, text_threshold, low_text, 0.7f);
+    det_front_threshold_kernel<__nv_bfloat16><<<n_pages, 256, 0, st>>>(hist, thr, n_pix, text_threshold, low_text, 0.7f, page_tab, WO);
     if (int rc = launch_ok()) return rc;
-    det_front_mask_kernel<__nv_bfloat16><<<g3, 256, 0, st>>>((const __nv_bfloat16*)map16, thr, mask, n_pix);
+    det_front_mask_kernel<__nv_bfloat16><<<g3, 256, 0, st>>>((const __nv_bfloat16*)map16, thr, mask, n_pix, page_tab, WO);
   }
   return launch_ok();
 }

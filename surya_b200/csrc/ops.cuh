@@ -105,7 +105,11 @@ int det_normalize_u8(int dtype, const unsigned char* in, void* out, int B, int H
 // top-10 % mean -> dynamic thresholds, binarised mask.  hist: B x 16384 zeroed uint32 scratch (left zeroed); thr: B x 4 floats
 // (text_threshold, low_text, top-10 % mean, scaling factor).
 int det_text_front(int dtype, const void* logits, int n_labels, int B, int hs, int ws, int HO, int WO, void* map16,
-                   unsigned char* mask, float* thr, unsigned int* hist, float text_threshold, float low_text, cudaStream_t st);
+                   unsigned char* mask, float* thr, unsigned int* hist, float text_threshold, float low_text, cudaStream_t st,
+                   const int* chunk_tab = nullptr, int n_pages = 0, const int* page_tab = nullptr, int max_page_rows = 0);
+// Page preparation (page_prep.cu): n_steps launches of the chained reduce / Lanczos jobs planned by surya_b200/page_prep.py.
+int det_page_resize(const unsigned char* pages, unsigned char* scratch, unsigned char* out, const long long* desc, const int* tables,
+                    int n_steps, const int* step_jobs, const long long* step_max_px, cudaStream_t st);
 // Back half on the device (det_boxes.cu): connected components, keep filter and dilated row extents as per-page tables
 // (layout in include/surya_b200.h, sb_det_text_boxes).
 size_t det_text_boxes_scratch_bytes(int B, int H, int W, int max_points);

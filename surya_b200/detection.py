@@ -321,6 +321,50 @@ class DetEngine:
                                          ptr(out["peak"]), ptr(out["points"]), stream_ptr()), "sb_det_text_boxes")
         return out
 
+    def page_resize(self, pages_dev: torch.Tensor, plan, processor_size: Tuple[int, int], out: torch.Tensor | None = None) -> torch.Tensor:
+        """sb_det_page_resize: the packed uint8 pages of `plan` (a page_prep.PagePlan) on the device -> processor-size uint8 chunks
+        [n_chunks, H, W, 3], byte-equal to split_image + prepare_image's PIL chain.  processor_size = (width, height)."""
+        pw, ph = processor_size
+        dev = pages_dev.device
+        n = len(plan.chunks)
+        if out is None:
+            out = torch.empty((n, ph, pw, 3), dtype=torch.uint8, device=dev)
+        scratch = getattr(self, "_resize_scratch", None)
+        if plan.scratch_bytes and (scratch is None or scratch.numel() < plan.scratch_bytes):
+            scratch = torch.empty((plan.scratch_bytes,), dtype=torch.uint8, device=dev)
+            self._resize_scratch = scratch
+        desc = torch.from_numpy(plan.desc).to(dev, non_blocking=True)
+        tables = torch.from_numpy(plan.tables).to(dev, non_blocking=True)
+        steps = len(plan.step_jobs)
+        check(self.lib.sb_det_page_resize(ptr(pages_dev), ptr(scratch if plan.scratch_bytes else None), ptr(out), ptr(desc),
+                                          ptr(tables), c_int(steps), (c_int * steps)(*plan.step_jobs),
+                                          (ctypes.c_longlong * steps)(*plan.step_max_px), stream_ptr()), "sb_det_page_resize")
+        return out
+
+    def text_front_stitched(self, logits: torch.Tensor, plan, size: Tuple[int, int], text_threshold: float = 0.6,
+                            low_text: float = 0.35) -> Dict[str, torch.Tensor]:
+        """text_front over the chunks of `plan`, stitched per page (sb_det_text_front_stitched): {"map": [rows, W] packed over
+        the pages (page p at rows plan.page_tab[p, 0] ...), "mask": same, "thr": [n_pages, 4]}.  size = (H, W) of a chunk."""
+        n, L, hs, ws = logits.shape
+        H, W = size
+        dev = logits.device
+        P = plan.page_tab.shape[0]
+        rows = int(plan.page_tab[:, 1].sum())
+        out = {"map": torch.empty((rows, W), dtype=logits.dtype, device=dev), "mask": torch.empty((rows, W), dtype=torch.uint8, device=dev),
+               "thr": torch.empty((P, 4), dtype=torch.float32, device=dev)}
+        hist = getattr(self, "_front_hist", None)
+        if hist is None or hist.shape[0] < P:
+            hist = torch.zeros((max(P, self.max_batch), 16384), dtype=torch.int32, device=dev)
+            self._front_hist = hist
+        chunk_tab = torch.from_numpy(plan.chunk_tab).to(dev, non_blocking=True)
+        page_tab = torch.from_numpy(plan.page_tab).to(dev, non_blocking=True)
+        check(self.lib.sb_det_text_front_stitched(c_int(dt_code(logits.dtype)), ptr(logits.contiguous()), c_int(L), c_int(n), c_int(hs),
+                                                  c_int(ws), c_int(H), c_int(W), ptr(chunk_tab), c_int(P), ptr(page_tab),
+                                                  c_int(int(plan.page_tab[:, 1].max())), ptr(out["map"]), ptr(out["mask"]),
+                                                  ptr(out["thr"]), ptr(hist), ctypes.c_float(text_threshold),
+                                                  ctypes.c_float(low_text), stream_ptr()), "sb_det_text_front_stitched")
+        return out
+
     def debug_buffer(self, name: str, B: int, H: int, W: int, C: int) -> torch.Tensor:
         idx = self.prog.buf_names.index(name)
         out = torch.empty((B, H, W, C), dtype=self.dtype, device=self.device)
@@ -600,3 +644,93 @@ def text_boxes_from_tables(box, peak, points, count: int):
     if max_confidence > 0:
         confidences = [c / max_confidence for c in confidences]
     return det, confidences
+
+
+@dataclass
+class PageDetection:
+    """Text lines of one page as DetectionPredictor.__call__ reports them (parallel_get_boxes, surya/detection/heatmap.py:156-186):
+    polygons and confidences in page coordinates, image_bbox = [0, 0, width, height], and the stitched heatmap's (width, height)."""
+    polygons: List[List[List[int]]]
+    confidences: List[float]
+    image_bbox: List[int]
+    heatmap_size: Tuple[int, int]
+
+
+def _page_groups(sizes, ph: int, chunk: int) -> List[List[int]]:
+    """Consecutive pages whose chunks fit one device round of at most `chunk` chunks (a page with more chunks goes alone)."""
+    from .page_prep import split_plan
+
+    groups, cur, n = [], [], 0
+    for i, (_, h) in enumerate(sizes):
+        k = len(split_plan(h, ph))
+        if cur and n + k > chunk:
+            groups.append(cur)
+            cur, n = [], 0
+        cur.append(i)
+        n += k
+    if cur:
+        groups.append(cur)
+    return groups
+
+
+def detect_text_pages(engine: DetEngine, pages, processor_size: Tuple[int, int], chunk: int = 16, text_threshold: float = 0.6,
+                      low_text: float = 0.35, max_boxes: int = DEFAULT_MAX_BOXES, max_points: int = DEFAULT_MAX_POINTS,
+                      max_chunks: int | None = None, max_page_pixels: int | None = None) -> List[PageDetection]:
+    """DetectionPredictor.__call__ (surya/detection/__init__.py:27-151 + parallel_get_boxes) for uint8 RGB pages [h, w, 3] of any
+    size, everything up to the minimum-area rectangles on the device: the pages go up as they are (3 bytes per pixel, one packed
+    pinned upload per round), sb_det_page_resize cuts tall pages into chunks and resizes them exactly like split_image +
+    prepare_image, the engine runs on the chunks, sb_det_text_front_stitched stitches each page's chunk heatmaps and thresholds
+    the whole page, sb_det_text_boxes extracts its lines at the page's stitched height.  processor_size = (width, height), a
+    multiple of 32 within the engine's max_hw.  Raises SuryaB200Error for a page beyond max_page_pixels or max_chunks."""
+    import numpy as np
+
+    from . import page_prep as pp
+    from .pipeline import page_polygons
+
+    pw, ph = processor_size
+    if ph > engine.max_hw[0] or pw > engine.max_hw[1] or ph % 32 or pw % 32:
+        raise _lib.SuryaB200Error(f"processor size {pw}x{ph} must be a multiple of 32 within {engine.max_hw[::-1]}")
+    pages = [np.ascontiguousarray(p) for p in pages]
+    for i, p in enumerate(pages):
+        if p.dtype != np.uint8 or p.ndim != 3 or p.shape[2] != 3:
+            raise _lib.SuryaB200Error(f"page {i} must be uint8 [h, w, 3], got {p.dtype} {list(p.shape)}")
+    sizes = [(p.shape[1], p.shape[0]) for p in pages]
+    limits = {"max_chunks": max_chunks or pp.DEFAULT_MAX_CHUNKS, "max_page_pixels": max_page_pixels or pp.DEFAULT_MAX_PAGE_PIXELS}
+    pp.plan_pages(sizes, processor_size, **limits)             # every page is checked before any work starts
+    dev = engine.device
+    out: List[PageDetection] = []
+    for group in _page_groups(sizes, ph, chunk):
+        plan = pp.plan_pages([sizes[i] for i in group], processor_size, **limits)
+        up = torch.empty((int(plan.page_off[-1]),), dtype=torch.uint8).pin_memory()
+        upn = up.numpy()
+        for j, i in enumerate(group):
+            upn[plan.page_off[j]:plan.page_off[j + 1]] = pages[i].reshape(-1)
+        chunks = engine.page_resize(up.to(dev, non_blocking=True), plan, processor_size)
+        logits = engine.forward(engine.normalize_u8(chunks))
+        front = engine.text_front_stitched(logits, plan, (ph, pw), text_threshold, low_text)
+        P = len(group)
+        tabs = box_tables(P, max_boxes, max_points, device=dev)
+        j = 0
+        while j < P:                       # pages of equal stitched height share a launch
+            r0, rows = (int(v) for v in plan.page_tab[j])
+            k = j + 1
+            while k < P and int(plan.page_tab[k, 1]) == rows:
+                k += 1
+            n = k - j
+            sub = {"map": front["map"][r0:r0 + n * rows].view(n, rows, pw), "mask": front["mask"][r0:r0 + n * rows].view(n, rows, pw),
+                   "thr": front["thr"][j:k]}
+            engine.text_boxes(sub, max_boxes, max_points, out={name: t[j:k] for name, t in tabs.items()})
+            j = k
+        host = {name: t.cpu() for name, t in tabs.items()}
+        thr = front["thr"].cpu()
+        for j, i in enumerate(group):
+            r0, rows = (int(v) for v in plan.page_tab[j])
+            if host["overflow"][j]:             # beyond the table capacity: finish the page on the host from its text front
+                boxes, conf = text_boxes_from_front(front["map"][r0:r0 + rows].float().cpu().numpy(),
+                                                    front["mask"][r0:r0 + rows].cpu().numpy(), float(thr[j, 0]), float(thr[j, 1]))
+            else:
+                boxes, conf = text_boxes_from_tables(host["box"][j].numpy(), host["peak"][j].numpy(), host["points"][j].numpy(),
+                                                     int(host["count"][j]))
+            polys, conf = page_polygons(boxes, conf, sizes[i], (pw, rows))
+            out.append(PageDetection(polys, conf, [0, 0, sizes[i][0], sizes[i][1]], (pw, rows)))
+    return out

@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import shard
-from .detection import DetEngine, detect_text_boxes_host
+from .detection import DetEngine, detect_text_boxes_host, detect_text_pages
 from .recognition import RecEngine, RecognitionRunner
 
 Y_EXPAND_MARGIN = 0.05      # settings.DETECTOR_BOX_Y_EXPAND_MARGIN
@@ -104,7 +104,8 @@ def slice_polygon(image: np.ndarray, poly: Sequence[Sequence[int]]) -> np.ndarra
 
 class OcrPipeline:
     """detect -> crop -> recognise over the CUDA engines.  `run(pages)` takes uint8 pages [N, H, W, 3] (H, W = the detection
-    processor size) and returns (lines grouped per page, timing breakdown in seconds)."""
+    processor size), or a list of uint8 pages [h, w, 3] of any size with optional high-resolution pages to crop from, and returns
+    (lines grouped per page, timing breakdown in seconds)."""
 
     def __init__(self, det: DetEngine, rec: RecEngine, rec_batch: int = 256, max_tokens: int = 128, det_chunk: int = 16,
                  workers: int = 16, math_mode: bool = True, preprocess: str = "host"):
@@ -124,15 +125,34 @@ class OcrPipeline:
         boxes = detect_text_boxes_host(self.det, pages_u8, chunk=self.det_chunk)
         return [page_polygons(b, c, (W, H), (W, H)) for b, c in boxes]
 
-    def run(self, pages: np.ndarray, fixed_steps: bool = False):
+    def detect_pages(self, pages: Sequence[np.ndarray], processor_size: Tuple[int, int]):
+        """uint8 pages of any size -> per page (polygons, confidences) in page coordinates (detect_text_pages)."""
+        return [(d.polygons, d.confidences) for d in detect_text_pages(self.det, pages, processor_size, chunk=self.det_chunk)]
+
+    def run(self, pages, fixed_steps: bool = False, highres_pages: Optional[Sequence[np.ndarray]] = None,
+            processor_size: Optional[Tuple[int, int]] = None):
+        """pages: uint8 [N, H, W, 3] at the detection processor size, or a list of uint8 [h, w, 3] pages of any size (resized and
+        split on the device; processor_size = (width, height), default the engine's max_hw).  With highres_pages (list form only;
+        an entry may be None for a page without one), each page's polygons are scaled to its high-resolution page with int(p * scale) and the crops are cut from it
+        (RecognitionPredictor.detect_and_slice_bboxes, surya/recognition/__init__.py:138-180); the returned line polygons stay in
+        the coordinates of the page given to detection."""
         t = {}
         t0 = time.perf_counter()
-        pages_t = torch.from_numpy(np.ascontiguousarray(pages))
-        if torch.cuda.is_available() and not pages_t.is_pinned():
-            pages_t = pages_t.pin_memory()
-        t["pin_pages"] = time.perf_counter() - t0
-        t0 = time.perf_counter()
-        det = self.detect(pages_t)
+        if isinstance(pages, np.ndarray):
+            if highres_pages is not None:
+                raise ValueError("highres_pages needs pages as a list")
+            pages_t = torch.from_numpy(np.ascontiguousarray(pages))
+            if torch.cuda.is_available() and not pages_t.is_pinned():
+                pages_t = pages_t.pin_memory()
+            t["pin_pages"] = time.perf_counter() - t0
+            t0 = time.perf_counter()
+            det = self.detect(pages_t)
+        else:
+            if highres_pages is not None and len(highres_pages) != len(pages):
+                raise ValueError(f"{len(highres_pages)} high-resolution pages for {len(pages)} pages")
+            if processor_size is None:
+                processor_size = (self.det.max_hw[1], self.det.max_hw[0])
+            det = self.detect_pages(pages, processor_size)
         t["detect(device + host boxes)"] = time.perf_counter() - t0
         t0 = time.perf_counter()
         lines: List[Line] = []
@@ -142,8 +162,13 @@ class OcrPipeline:
             # uint8 page first and converting only the crop gives the identical float values (integers, pad value 255) without
             # touching 12 MB per page; the device path keeps the crop as uint8
             img = pages[pg]
-            for p, c in zip(polys, conf):
-                crop = slice_polygon(img, p)
+            cut = polys
+            if highres_pages is not None and highres_pages[pg] is not None:
+                img = highres_pages[pg]
+                sx, sy = img.shape[1] / pages[pg].shape[1], img.shape[0] / pages[pg].shape[0]
+                cut = [[[int(x * sx), int(y * sy)] for x, y in p] for p in polys]
+            for p, q, c in zip(polys, cut, conf):
+                crop = slice_polygon(img, q)
                 if crop.shape[0] == 0 or crop.shape[1] == 0:
                     continue
                 if self.preprocess != "device":
@@ -170,16 +195,24 @@ class OcrPipeline:
         return per_page, t
 
 
-def sharded_ocr(pipe: OcrPipeline, pages: np.ndarray, max_tokens: int, device=None, fixed_steps: bool = False):
-    """Every rank runs `pipe` on its contiguous share of `pages` (identical array on all ranks, or any array whose rows this rank
-    owns are valid) and the per-line results are all-gathered: returns (lines per page for ALL pages, this rank's timings).
+def sharded_ocr(pipe: OcrPipeline, pages, max_tokens: int, device=None, fixed_steps: bool = False,
+                highres_pages: Optional[Sequence[np.ndarray]] = None, processor_size: Optional[Tuple[int, int]] = None):
+    """Every rank runs `pipe` on its contiguous share of `pages` (identical array or list on all ranks, or any whose pages this rank
+    owns are valid; a list may hold pages of any size, with optional highres_pages as in OcrPipeline.run) and the per-line
+    results are all-gathered: returns (lines per page for ALL pages, this rank's timings).
     Exchange format: per page up to `cap` lines of [polygon 8, confidence, n_tokens, tokens max_tokens] packed as int32 / fp32."""
     import torch.distributed as dist
 
     rank, n_ranks = shard.world()
     slices = shard.page_slices(len(pages), n_ranks)
     lo, hi = slices[rank]
-    per_page, timings = pipe.run(pages[lo:hi], fixed_steps=fixed_steps) if hi > lo else ([], {})
+    if hi <= lo:
+        per_page, timings = [], {}
+    elif isinstance(pages, np.ndarray):
+        per_page, timings = pipe.run(pages[lo:hi], fixed_steps=fixed_steps)
+    else:
+        per_page, timings = pipe.run(list(pages[lo:hi]), fixed_steps=fixed_steps, processor_size=processor_size,
+                                     highres_pages=None if highres_pages is None else list(highres_pages[lo:hi]))
     if n_ranks == 1:
         return per_page, timings
     dev = shard._collective_device(device)
