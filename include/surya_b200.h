@@ -419,6 +419,16 @@ int sb_box_next_token(const float* bbox, const float* const* heads, const int* h
                       float bbox_size, long long* out, unsigned char* done, int done_head, int eos, int pad, int B, int* cache_pos,
                       const int* hist_base, int hist_T, long long* hist_tok, float* hist_bbox, float* const* hist_heads,
                       unsigned char* hist_done, void* stream);
+/* sb_box_next_token with LayoutPredictor's header/footer rule (see sb_layout_decode_pages) on head 0, which must be an argmax
+ * head: page_wh int32 [B, 2] (device, required), sticky u8 [B] (device, may be NULL) = rows already done, skipped by the rule;
+ * header / footer = the class tokens of PageHeader / PageFooter; dtype = the model dtype (SB_DT_*) the polygon is rounded to.
+ * done_head must be 0: done comes from the class head, and rows done at this step are not relabelled.
+ * The rule's modified logits go to hist_heads[0]. */
+int sb_box_next_token_pages(const float* bbox, const float* const* heads, const int* head_n, const int* head_mode, int n_heads,
+                            float bbox_size, long long* out, unsigned char* done, int done_head, int eos, int pad, int B,
+                            int* cache_pos, const int* hist_base, int hist_T, long long* hist_tok, float* hist_bbox,
+                            float* const* hist_heads, unsigned char* hist_done, const int* page_wh, const unsigned char* sticky,
+                            int dtype, int header, int footer, float skew_scaler, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ layout / table_rec engine
  * Donut-Swin encoder + ADETR box decoder with the layer loops, workspaces, K/V caches and the greedy loop in C++
@@ -457,6 +467,8 @@ typedef struct sb_layout_config {
    *   max_rows            decoder rows and self-attention caches
    *   max_prefill_tokens  prompt tokens per batched prefill chunk (the decoder activations hold max(max_rows, this) rows) */
   int max_rows, max_prefill_tokens;
+  /* read by sb_layout_decode_pages only: special_token_count and skew_scaler of the layout decoder config */
+  int special_tokens, skew_scaler;
 } sb_layout_config;
 typedef struct sb_layout_engine sb_layout_engine;
 
@@ -472,6 +484,31 @@ int sb_layout_encode(sb_layout_engine* e, const void* pixels, int pixels_f32, in
 int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long long* prompt, int q_len, int n_steps,
                      long long* hist_tok, float* hist_bbox, float* const* hist_heads, unsigned char* hist_done, int use_graph,
                      void* stream);
+/* LayoutPredictor's decode loop (surya/layout/__init__.py:106-183) on the device: sb_layout_decode's greedy pass plus the
+ * predictor's rules, layout engines only.
+ *   header/footer rule (:147-174): a row not yet done whose class is PageHeader / PageFooter gets its polygon computed as
+ *     prediction_to_polygon (surya/layout/util.py:4-40) does from the model-dtype row [bbox * bbox_size, class]; when corner 0
+ *     is below 0.8 and corner 2 above 0.2 of its page size page_wh[b] = (w, h) (device int32 [batch, 2]) on both axes, that
+ *     class logit is set to 0 and the first maximum taken again.  The new class feeds the next step and the modified logits
+ *     are what hist_cls keeps.
+ *   stop rule (:129-135): a row is done from its first step whose first argmax is eos or pad (sticky); the loop stops after
+ *     the first group of 8 steps at which every row is done.
+ * Histories (device): tok [n_steps, batch, 7] i64, bbox [n_steps, batch, 6] f32, hist_cls [n_steps, batch, label_count] f32,
+ * done [n_steps, batch] u8 (this step's done flag, not sticky).  *n_run_host = the steps whose histories were written (>= the
+ * step at which the last row became done; n_steps when some row never does).  page_wh must stay valid until the next call
+ * with other buffers: the step graphs read it. */
+int sb_layout_decode_pages(sb_layout_engine* e, const void* enc, int batch, const long long* prompt, int q_len, const int* page_wh,
+                           int n_steps, long long* hist_tok, float* hist_bbox, float* hist_cls, unsigned char* hist_done,
+                           int* n_run_host, void* stream);
+/* SuryaEncoderImageProcessor.process_inner (surya/common/donut/processor.py:61-116) on the device, for layout and table_rec:
+ * cv2.resize(INTER_CUBIC, since the processor's resample 2 is cv2's INTER_CUBIC) of a uint8 RGB rectangle to out_w x out_h,
+ * then x * (1/255) (double -> float), (x - 0.5) / 0.5 in float and the cast to `dtype` (fp16 / bf16), NCHW into out.
+ * pages: uint8 HWC images packed in one buffer.  jobs int64 [n_jobs, 8]: byte offset of the page, page width (row pitch in
+ * pixels), x0, y0 of the source rectangle, x and y tap-table rows, output row, 0.  Tap tables [rows, 4]: tap_idx int32 = source
+ * column / row relative to the rectangle (already clamped to it), tap_w float32 = cubic weight; a table for an axis of n
+ * source pixels scaled to m has m rows (surya_b200/layout_pages.py builds and caches them). */
+int sb_layout_preprocess(int dtype, const unsigned char* pages, const long long* jobs, int n_jobs, const int* tap_idx,
+                         const float* tap_w, int out_h, int out_w, void* out, void* stream);
 /* table_rec two-pass flow (TableRecPredictor.batch_table_recognition, surya/table_rec/__init__.py:134-236).
  * sb_layout_cross_kv projects the cross-attention K/V of every decoder layer for n_tables <= max_batch encoder states
  * enc [n_tables, Lk, enc_hidden] and holds them.  sb_layout_decode writes the same buffers: after it runs, the held K/V are

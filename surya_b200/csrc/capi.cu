@@ -176,4 +176,21 @@ int sb_box_next_token(const float* bbox, const float* const* heads, const int* h
                         hist_base, hist_T, hist_tok, hist_bbox, hist_heads, hist_done, static_cast<cudaStream_t>(stream));
 }
 
+int sb_box_next_token_pages(const float* bbox, const float* const* heads, const int* head_n, const int* head_mode, int n_heads,
+                            float bbox_size, long long* out, unsigned char* done, int done_head, int eos, int pad, int B,
+                            int* cache_pos, const int* hist_base, int hist_T, long long* hist_tok, float* hist_bbox,
+                            float* const* hist_heads, unsigned char* hist_done, const int* page_wh, const unsigned char* sticky,
+                            int dtype, int header, int footer, float skew_scaler, void* stream) {
+  if (!page_wh) { set_error("sb_box_next_token_pages: null page_wh (sb_box_next_token has no page rule)"); return -1; }
+  if (n_heads < 1 || done_head != 0) {
+    set_error("sb_box_next_token_pages: the page rule needs the class head as head 0 and done from it (done_head 0)");
+    return -1;
+  }
+  if (dtype != DT_F16 && dtype != DT_BF16) { set_error("sb_box_next_token_pages: dtype must be fp16 or bf16"); return -1; }
+  PageRule r;
+  r.page_wh = page_wh; r.sticky = sticky; r.dtype = dtype; r.header = header; r.footer = footer; r.skew_scaler = skew_scaler;
+  return box_next_token(bbox, heads, head_n, head_mode, n_heads, bbox_size, out, done, done_head, eos, pad, B, cache_pos,
+                        hist_base, hist_T, hist_tok, hist_bbox, hist_heads, hist_done, static_cast<cudaStream_t>(stream), r);
+}
+
 }  // extern "C"

@@ -56,6 +56,7 @@ struct sb_layout_engine {
   // decode loop: GRAPH_GROUP steps per replay, and one step for the tail
   StepGraph g_group{"sb_layout_decode", GRAPH_GROUP}, g_one{"sb_layout_decode", 1};
   StepGraph g_rows{"sb_layout_decode_rows", GRAPH_GROUP}, g_rows_one{"sb_layout_decode_rows", 1};
+  StepGraph g_pages{"sb_layout_decode_pages", GRAPH_GROUP}, g_pages_one{"sb_layout_decode_pages", 1};
   EngineStream stream;
 
   ~sb_layout_engine() {
@@ -214,16 +215,62 @@ static int run_token(sb_layout_engine* e, const long long* tok, const int* pos, 
   return 0;
 }
 
+// rule: LayoutPredictor's header/footer relabelling and its done flags (sb_layout_decode_pages); null for the plain greedy loop
 static int run_next(sb_layout_engine* e, int B, int hist_T, long long* hist_tok, float* hist_bbox, float* const* hist_heads,
-                    unsigned char* hist_done, cudaStream_t st) {
+                    unsigned char* hist_done, cudaStream_t st, const PageRule* rule = nullptr) {
   const sb_layout_config& c = e->c;
   const float* heads[4];
   int hn[4], hm[4];
   for (int k = 0; k < c.n_out_heads; ++k) { heads[k] = e->out_head[k]; hn[k] = c.head_n[k]; hm[k] = 0; }
   if (c.kind == 1) hm[2] = 1;   // colspan: round(max(v, 1))
   return box_next_token(e->out_bbox, heads, hn, hm, c.n_out_heads, static_cast<float>(c.bbox_size), e->tok, e->done,
-                        c.kind == 1 ? 0 : -1, c.eos, c.pad, B, e->pos, e->base, hist_T, hist_tok, hist_bbox, hist_heads, hist_done,
-                        st);
+                        (c.kind == 1 || rule) ? 0 : -1, c.eos, c.pad, B, e->pos, e->base, hist_T, hist_tok, hist_bbox, hist_heads,
+                        hist_done, st, rule ? *rule : PageRule());
+}
+
+// Pinned active-row counts and their events, created on first use by the loops that stop early.
+static int ensure_active_count(sb_layout_engine* e, const char* who) {
+  if (e->h_active) return 0;
+  if (cudaHostAlloc(&e->h_active, 2 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) {
+    cudaGetLastError(); e->h_active = nullptr; set_error("%s: pinned allocation failed", who); return -8;
+  }
+  for (cudaEvent_t& ev : e->ev_active)
+    if (!ev && cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
+      cudaGetLastError(); ev = nullptr; set_error("%s: event creation failed", who); return -8;
+    }
+  return 0;
+}
+
+// The `left` steps after the first, as replays of `group` (GRAPH_GROUP steps) and `one`, each step ending in rows_done_count.
+// Early exit: after each group the active-row count goes to pinned memory.  Group g+1 is enqueued before the count of group g
+// is read, so the GPU never waits for the host; when that count is 0, group g+1's steps are extra and the loop stops.
+// *ran += the steps enqueued.
+static int replay_until_done(sb_layout_engine* e, StepGraph& group, StepGraph& one, int left, cudaStream_t st, int* ran,
+                             const char* who) {
+  const int groups = left / GRAPH_GROUP;
+  bool stop = false;
+  auto post = [&](int g) -> int {
+    if (cudaMemcpyAsync(e->h_active + (g & 1), e->n_active, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaEventRecord(e->ev_active[g & 1], st) != cudaSuccess) {
+      cudaGetLastError(); set_error("%s: active-count copy failed", who); return -5;
+    }
+    return 0;
+  };
+  auto all_done = [&](int g) { cudaEventSynchronize(e->ev_active[g & 1]); return e->h_active[g & 1] == 0; };
+  for (int g = 0; g < groups && !stop; ++g) {
+    CK(group.replay(1, st));
+    *ran += GRAPH_GROUP;
+    CK(post(g));
+    if (g > 0 && all_done(g - 1)) stop = true;
+  }
+  if (!stop && left % GRAPH_GROUP) {
+    if (groups > 0 && all_done(groups - 1)) stop = true;
+    if (!stop) {
+      CK(one.replay(left % GRAPH_GROUP, st));
+      *ran += left % GRAPH_GROUP;
+    }
+  }
+  return 0;
 }
 
 extern "C" {
@@ -319,15 +366,18 @@ int sb_layout_encode(sb_layout_engine* e, const void* pixels, int pixels_f32, in
   return run_encoder(e, pixels, pixels_f32, batch, enc_out, static_cast<cudaStream_t>(stream));
 }
 
-int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long long* prompt, int q_len, int n_steps,
-                     long long* hist_tok, float* hist_bbox, float* const* hist_heads, unsigned char* hist_done, int use_graph,
-                     void* stream) {
-  if (!e || !enc || !prompt || !hist_tok) { set_error("sb_layout_decode: null argument"); return -1; }
+// The greedy pass of sb_layout_decode, and with `rule` (sb_layout_decode_pages) LayoutPredictor's loop: the header/footer rule in
+// the token step, sticky done flags and the early exit after the first group of steps at which every row is done (*n_run = the
+// steps that ran).  Without a rule every one of the n_steps steps runs.
+static int greedy_decode(sb_layout_engine* e, const char* who, const void* enc, int batch, const long long* prompt, int q_len,
+                         int n_steps, long long* hist_tok, float* hist_bbox, float* const* hist_heads, unsigned char* hist_done,
+                         int use_graph, void* stream, const PageRule* rule, int* n_run) {
   const sb_layout_config& c = e->c;
-  if (batch <= 0 || batch > c.max_batch) { set_error("sb_layout_decode: batch %d outside 1..%d", batch, c.max_batch); return -2; }
-  if (q_len < 1 || n_steps < 1 || q_len - 1 + n_steps > c.s_max) { set_error("sb_layout_decode: prompt + steps exceed s_max %d", c.s_max); return -3; }
+  if (batch <= 0 || batch > c.max_batch) { set_error("%s: batch %d outside 1..%d", who, batch, c.max_batch); return -2; }
+  if (q_len < 1 || n_steps < 1 || q_len - 1 + n_steps > c.s_max) { set_error("%s: prompt + steps exceed s_max %d", who, c.s_max); return -3; }
+  if (rule) CK(ensure_active_count(e, who));
   Hop hop(e->stream, static_cast<cudaStream_t>(stream), use_graph);
-  if (hop.failed) { set_error("sb_layout_decode: could not create the engine stream"); return -8; }
+  if (hop.failed) { set_error("%s: could not create the engine stream", who); return -8; }
   const cudaStream_t st = hop.st;
 
   const int B = batch, ncol = e->ncol();
@@ -336,7 +386,7 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
   // encoder states -> persistent buffer; cross-attention K/V of every layer (SuryaADETRDecoderSdpaCrossAttention caches them at
   // the first call, adetr/decoder.py:150-194)
   if (cudaMemcpyAsync(e->enc, enc, static_cast<size_t>(B) * e->Lk * c.enc_hidden * es, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-    cudaGetLastError(); set_error("sb_layout_decode: encoder copy failed"); return -4;
+    cudaGetLastError(); set_error("%s: encoder copy failed", who); return -4;
   }
   const int KVW = 2 * c.n_kv * c.head_dim;
   for (int l = 0; l < c.dec_layers; ++l)
@@ -348,11 +398,11 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
     // gather column j of the prompt [B, q_len, ncol] into the token buffer
     if (cudaMemcpy2DAsync(e->tok, ncol * sizeof(long long), prompt + static_cast<size_t>(j) * ncol, static_cast<size_t>(q_len) * ncol * sizeof(long long),
                           ncol * sizeof(long long), B, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-      cudaGetLastError(); set_error("sb_layout_decode: prompt copy failed"); return -5;
+      cudaGetLastError(); set_error("%s: prompt copy failed", who); return -5;
     }
     for (int b = 0; b < B; ++b) hpos[b] = j;
     if (cudaMemcpyAsync(e->pos, hpos.data(), B * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess) {
-      cudaGetLastError(); set_error("sb_layout_decode: position copy failed"); return -5;
+      cudaGetLastError(); set_error("%s: position copy failed", who); return -5;
     }
     if (j == q_len - 1) break;
     cudaStreamSynchronize(st);     // hpos is reused by the next iteration (pageable source)
@@ -360,30 +410,74 @@ int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long
   }
   const int base = q_len - 1;
   if (cudaMemcpyAsync(e->base, &base, sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess) {
-    cudaGetLastError(); set_error("sb_layout_decode: base copy failed"); return -5;
+    cudaGetLastError(); set_error("%s: base copy failed", who); return -5;
+  }
+  if (rule && cudaMemsetAsync(e->sticky, 0, B, st) != cudaSuccess) {
+    cudaGetLastError(); set_error("%s: done-flag reset failed", who); return -5;
   }
   cudaStreamSynchronize(st);       // host sources above are stack / vector memory
 
   auto body = [&](cudaStream_t s) -> int {
     CK(run_token(e, e->tok, e->pos, B, s));
-    return run_next(e, B, n_steps, hist_tok, hist_bbox, hist_heads, hist_done, s);
+    CK(run_next(e, B, n_steps, hist_tok, hist_bbox, hist_heads, hist_done, s, rule));
+    return rule ? rows_done_count(e->done, e->sticky, e->n_active, B, s) : 0;
   };
   CK(body(st));                    // first step eagerly (sets kernel attributes before any capture)
+  if (n_run) *n_run = 1;
   int left = n_steps - 1;
   if (left <= 0) return 0;
+  StepGraph& group = rule ? e->g_pages : e->g_group;
+  StepGraph& one = rule ? e->g_pages_one : e->g_one;
   if (!use_graph) {
     for (int i = 0; i < left; ++i) CK(body(st));
+    if (n_run) *n_run = n_steps;
     return 0;
   }
   const StepGraph::Key key = {hist_tok, hist_bbox, hist_done, hist_heads ? hist_heads[0] : nullptr,
-                              reinterpret_cast<const void*>(static_cast<uintptr_t>(n_steps))};
-  if (!e->g_group.hit(key, B) || !e->g_one.hit(key, B)) {
-    CK(e->g_group.capture(key, B, st, body));
-    CK(e->g_one.capture(key, B, st, body));
+                              reinterpret_cast<const void*>(static_cast<uintptr_t>(n_steps)), rule ? rule->page_wh : nullptr};
+  if (!group.hit(key, B) || !one.hit(key, B)) {
+    CK(group.capture(key, B, st, body));
+    CK(one.capture(key, B, st, body));
   }
-  CK(e->g_group.replay(left / GRAPH_GROUP, st));
-  return e->g_one.replay(left % GRAPH_GROUP, st);
+  if (rule) return replay_until_done(e, group, one, left, st, n_run, who);
+  CK(group.replay(left / GRAPH_GROUP, st));
+  return one.replay(left % GRAPH_GROUP, st);
 }
+
+int sb_layout_decode(sb_layout_engine* e, const void* enc, int batch, const long long* prompt, int q_len, int n_steps,
+                     long long* hist_tok, float* hist_bbox, float* const* hist_heads, unsigned char* hist_done, int use_graph,
+                     void* stream) {
+  if (!e || !enc || !prompt || !hist_tok) { set_error("sb_layout_decode: null argument"); return -1; }
+  return greedy_decode(e, "sb_layout_decode", enc, batch, prompt, q_len, n_steps, hist_tok, hist_bbox, hist_heads, hist_done,
+                       use_graph, stream, nullptr, nullptr);
+}
+
+int sb_layout_decode_pages(sb_layout_engine* e, const void* enc, int batch, const long long* prompt, int q_len, const int* page_wh,
+                           int n_steps, long long* hist_tok, float* hist_bbox, float* hist_cls, unsigned char* hist_done,
+                           int* n_run_host, void* stream) {
+  if (!e || !enc || !prompt || !page_wh || !hist_tok || !hist_bbox || !hist_cls || !hist_done || !n_run_host) {
+    set_error("sb_layout_decode_pages: null argument");
+    return -1;
+  }
+  *n_run_host = 0;
+  const sb_layout_config& c = e->c;
+  if (c.kind != 0) { set_error("sb_layout_decode_pages: needs a layout engine (the page rule reads the layout class head)"); return -2; }
+  // PageHeader / PageFooter are label ids 10 / 9 (surya/layout/model/config.py:16-34), after the special tokens
+  if (c.special_tokens < 0 || c.special_tokens + 10 >= c.head_n[0]) {
+    set_error("sb_layout_decode_pages: %d special tokens and %d classes leave no PageHeader class", c.special_tokens, c.head_n[0]);
+    return -2;
+  }
+  PageRule rule;
+  rule.page_wh = page_wh; rule.sticky = e->sticky; rule.dtype = c.dtype;
+  rule.header = 10 + c.special_tokens; rule.footer = 9 + c.special_tokens; rule.skew_scaler = static_cast<float>(c.skew_scaler);
+  float* heads[1] = {hist_cls};
+  int ran = 0;
+  CK(greedy_decode(e, "sb_layout_decode_pages", enc, batch, prompt, q_len, n_steps, hist_tok, hist_bbox, heads, hist_done, 1, stream,
+                   &rule, &ran));
+  *n_run_host = ran;
+  return 0;
+}
+
 
 int sb_layout_cross_kv(sb_layout_engine* e, const void* enc, int n_tables, void* stream) {
   if (!e || !enc) { set_error("sb_layout_cross_kv: null argument"); return -1; }
@@ -457,15 +551,7 @@ int sb_layout_decode_rows(sb_layout_engine* e, const int* row_table_host, int ro
       set_error("sb_layout_decode_rows: row %d maps to table %d, outside the %d held tables", r, row_table_host[r], e->held_tables);
       return -4;
     }
-  if (!e->h_active) {
-    if (cudaHostAlloc(&e->h_active, 2 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) {
-      cudaGetLastError(); e->h_active = nullptr; set_error("sb_layout_decode_rows: pinned allocation failed"); return -8;
-    }
-    for (cudaEvent_t& ev : e->ev_active)
-      if (!ev && cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) {
-        cudaGetLastError(); ev = nullptr; set_error("sb_layout_decode_rows: event creation failed"); return -8;
-      }
-  }
+  CK(ensure_active_count(e, "sb_layout_decode_rows"));
   Hop hop(e->stream, static_cast<cudaStream_t>(stream), true);
   if (hop.failed) { set_error("sb_layout_decode_rows: could not create the engine stream"); return -8; }
   const cudaStream_t st = hop.st;
@@ -525,30 +611,7 @@ int sb_layout_decode_rows(sb_layout_engine* e, const int* row_table_host, int ro
       CK(e->g_rows.capture(key, rows, st, body));
       CK(e->g_rows_one.capture(key, rows, st, body));
     }
-    // Early exit: after each group the active-row count goes to pinned memory.  Group g+1 is enqueued before the count of group g
-    // is read, so the GPU never waits for the host; when that count is 0, group g+1's steps are extra and the loop stops.
-    const int groups = left / GRAPH_GROUP;
-    bool stop = false;
-    auto post = [&](int g) -> int {
-      if (cudaMemcpyAsync(e->h_active + (g & 1), e->n_active, sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-          cudaEventRecord(e->ev_active[g & 1], st) != cudaSuccess)
-        return fail("active-count copy");
-      return 0;
-    };
-    auto all_done = [&](int g) { cudaEventSynchronize(e->ev_active[g & 1]); return e->h_active[g & 1] == 0; };
-    for (int g = 0; g < groups && !stop; ++g) {
-      CK(e->g_rows.replay(1, st));
-      ran += GRAPH_GROUP;
-      CK(post(g));
-      if (g > 0 && all_done(g - 1)) stop = true;
-    }
-    if (!stop && left % GRAPH_GROUP) {
-      if (groups > 0 && all_done(groups - 1)) stop = true;
-      if (!stop) {
-        CK(e->g_rows_one.replay(left % GRAPH_GROUP, st));
-        ran += left % GRAPH_GROUP;
-      }
-    }
+    CK(replay_until_done(e, e->g_rows, e->g_rows_one, left, st, &ran, "sb_layout_decode_rows"));
   }
   *n_run_host = ran;
   return 0;

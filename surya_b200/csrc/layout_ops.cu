@@ -706,13 +706,41 @@ int label_embed(int dtype, const long long* boxes, const void* const* tables, vo
 // is eos or pad (table_rec/__init__.py:84-87).  Optional decode-loop state so that a whole step can live in a CUDA graph:
 // cache_pos[b] is advanced (decoder_position_ids + 1) and the step's tokens / raw head outputs are appended to history
 // arrays at row (cache_pos[b] - hist_base[0]).
+// Optional page rule (rule.page_wh non-null): LayoutPredictor's header/footer relabelling (layout/__init__.py:147-174) on head 0.
 struct StepHeads { const float* p[4]; int n[4]; int mode[4]; float* hist[4]; };
+
+// rounding of one torch op on 16-bit CPU tensors: the float result rounded to the model dtype
+__device__ __forceinline__ float round_dt(float v, int dtype) {
+  return dtype == DT_F16 ? __half2float(__float2half_rn(v)) : __bfloat162float(__float2bfloat16_rn(v));
+}
+
+// prediction_to_polygon (layout/util.py:4-40) from the model-dtype row [bbox * bbox_size x6, class] that the predictor builds
+// (layout/__init__.py:127, 137), then the position test of the rule in Python float (double): corner 0 below 0.8 and corner 2
+// above 0.2 of the page on both axes.
+__device__ __forceinline__ bool header_footer_misplaced(const float* bb, float bbox_size, const PageRule& r, int b) {
+  float v[6];
+#pragma unroll
+  for (int i = 0; i < 6; ++i) v[i] = round_dt(__fmul_rn(bb[i], bbox_size), r.dtype);
+  const float hw = round_dt(__fdiv_rn(v[2], 2.f), r.dtype), hh = round_dt(__fdiv_rn(v[3], 2.f), r.dtype);
+  const float x1 = round_dt(__fsub_rn(v[0], hw), r.dtype), x2 = round_dt(__fadd_rn(v[0], hw), r.dtype);
+  const float y1 = round_dt(__fsub_rn(v[1], hh), r.dtype), y2 = round_dt(__fadd_rn(v[1], hh), r.dtype);
+  const float sx = floorf(round_dt(__fdiv_rn(round_dt(__fsub_rn(v[4], r.skew_scaler), r.dtype), 2.f), r.dtype));
+  const float sy = floorf(round_dt(__fdiv_rn(round_dt(__fsub_rn(v[5], r.skew_scaler), r.dtype), 2.f), r.dtype));
+  // |skew| < skew_min -> 0 only ever clears a (signed) zero: the floors are integers
+  const double pw = r.page_wh[2 * b], ph = r.page_wh[2 * b + 1];
+  const double ws = pw / static_cast<double>(bbox_size), hs = ph / static_cast<double>(bbox_size);
+  const double p0x = static_cast<double>(round_dt(__fsub_rn(x1, sx), r.dtype)) * ws;
+  const double p0y = static_cast<double>(round_dt(__fsub_rn(y1, sy), r.dtype)) * hs;
+  const double p2x = static_cast<double>(round_dt(__fadd_rn(x2, sx), r.dtype)) * ws;
+  const double p2y = static_cast<double>(round_dt(__fadd_rn(y2, sy), r.dtype)) * hs;
+  return p0y < ph * .8 && p2y > ph * .2 && p0x < pw * .8 && p2x > pw * .2;
+}
 
 __global__ void box_next_token_kernel(const float* __restrict__ bbox, StepHeads hd, int n_heads, float bbox_size,
                                       long long* __restrict__ out, unsigned char* __restrict__ done, int done_head, int eos,
                                       int pad, int B, int* __restrict__ cache_pos, const int* __restrict__ hist_base, int hist_T,
                                       long long* __restrict__ hist_tok, float* __restrict__ hist_bbox,
-                                      unsigned char* __restrict__ hist_done) {
+                                      unsigned char* __restrict__ hist_done, PageRule rule) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const int ncol = 6 + n_heads;
@@ -738,6 +766,21 @@ __global__ void box_next_token_kernel(const float* __restrict__ bbox, StepHeads 
     tok[6 + k] = t;
     if (k == done_head) dn = (t == eos || t == pad) ? 1 : 0;
   }
+  // header / footer rule: the class logit of a misplaced PageHeader / PageFooter is set to 0 and the first maximum taken again;
+  // the new class feeds the next step and the modified logits go to the history (done still comes from the first argmax)
+  long long zeroed = -1;
+  if (rule.page_wh && !dn && !(rule.sticky && rule.sticky[b]) && (tok[6] == rule.header || tok[6] == rule.footer) &&
+      header_footer_misplaced(bbox + static_cast<size_t>(b) * 6, bbox_size, rule, b)) {
+    const float* p = hd.p[0] + static_cast<size_t>(b) * hd.n[0];
+    zeroed = tok[6];
+    int best = 0;
+    float bv = zeroed == 0 ? 0.f : p[0];
+    for (int j = 1; j < hd.n[0]; ++j) {
+      const float v = j == zeroed ? 0.f : p[j];
+      if (v > bv) { bv = v; best = j; }
+    }
+    tok[6] = best;
+  }
   int row = -1;
   if (cache_pos) {
     const int pos = cache_pos[b];
@@ -752,7 +795,8 @@ __global__ void box_next_token_kernel(const float* __restrict__ bbox, StepHeads 
       for (int i = 0; i < 6; ++i) hist_bbox[r * 6 + i] = bbox[b * 6 + i];
     for (int k = 0; k < n_heads; ++k)
       if (hd.hist[k])
-        for (int j = 0; j < hd.n[k]; ++j) hd.hist[k][r * hd.n[k] + j] = hd.p[k][static_cast<size_t>(b) * hd.n[k] + j];
+        for (int j = 0; j < hd.n[k]; ++j)
+          hd.hist[k][r * hd.n[k] + j] = (k == 0 && j == zeroed) ? 0.f : hd.p[k][static_cast<size_t>(b) * hd.n[k] + j];
     if (hist_done && done_head >= 0) hist_done[r] = dn;
   }
   // the token buffer may alias nothing this step still reads: written last
@@ -763,16 +807,17 @@ __global__ void box_next_token_kernel(const float* __restrict__ bbox, StepHeads 
 int box_next_token(const float* bbox, const float* const* heads, const int* head_n, const int* head_mode, int n_heads,
                    float bbox_size, long long* out, unsigned char* done, int done_head, int eos, int pad, int B, int* cache_pos,
                    const int* hist_base, int hist_T, long long* hist_tok, float* hist_bbox, float* const* hist_heads,
-                   unsigned char* hist_done, cudaStream_t st) {
+                   unsigned char* hist_done, cudaStream_t st, const PageRule& rule) {
   if (B <= 0) return 0;
   if (n_heads < 0 || n_heads > 4) { set_error("box_next_token: at most 4 heads"); return -1; }
+  if (rule.page_wh && (n_heads < 1 || head_mode[0] != 0)) { set_error("box_next_token: the page rule needs an argmax class head 0"); return -1; }
   StepHeads h{};
   for (int i = 0; i < n_heads; ++i) {
     h.p[i] = heads[i]; h.n[i] = head_n[i]; h.mode[i] = head_mode[i];
     h.hist[i] = hist_heads ? hist_heads[i] : nullptr;
   }
   box_next_token_kernel<<<(B + 63) / 64, 64, 0, st>>>(bbox, h, n_heads, bbox_size, out, done, done_head, eos, pad, B, cache_pos,
-                                                      hist_base, hist_T, hist_tok, hist_bbox, hist_done);
+                                                      hist_base, hist_T, hist_tok, hist_bbox, hist_done, rule);
   return launch_ok();
 }
 

@@ -132,10 +132,19 @@ int attn_single_query(int dtype, const void* q, int ldq, const void* K, const vo
                       const int* kv_index = nullptr);
 int label_embed(int dtype, const long long* boxes, const void* const* tables, void* out, int n, int box_w, int prop_w,
                 int bbox_size, int vocab, cudaStream_t st);
+// LayoutPredictor's header/footer rule inside box_next_token (off when page_wh is null): page_wh int32 [B, 2] = (w, h) of the
+// image row b was preprocessed from; sticky (may be null) = rows already done, which the rule skips; header / footer = class
+// tokens of PageHeader / PageFooter (label id + special_token_count); dtype = the model dtype the polygon is rounded to.
+struct PageRule {
+  const int* page_wh = nullptr;
+  const unsigned char* sticky = nullptr;
+  int dtype = DT_F16, header = -1, footer = -1;
+  float skew_scaler = 0.f;
+};
 int box_next_token(const float* bbox, const float* const* heads, const int* head_n, const int* head_mode, int n_heads,
                    float bbox_size, long long* out, unsigned char* done, int done_head, int eos, int pad, int B, int* cache_pos,
                    const int* hist_base, int hist_T, long long* hist_tok, float* hist_bbox, float* const* hist_heads,
-                   unsigned char* hist_done, cudaStream_t st);
+                   unsigned char* hist_done, cudaStream_t st, const PageRule& rule = PageRule());
 // sticky[b] |= done[b]; n_active[0] = number of rows b < B with sticky[b] == 0 (table_rec early exit).
 int rows_done_count(const unsigned char* done, unsigned char* sticky, int* n_active, int B, cudaStream_t st);
 

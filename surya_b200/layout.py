@@ -40,6 +40,7 @@ class _LayoutCfgC(ctypes.Structure):
         ("eos", ctypes.c_int), ("pad", ctypes.c_int),
         ("max_batch", ctypes.c_int), ("s_max", ctypes.c_int),
         ("max_rows", ctypes.c_int), ("max_prefill_tokens", ctypes.c_int),
+        ("special_tokens", ctypes.c_int), ("skew_scaler", ctypes.c_int),
     ]
 
 
@@ -168,6 +169,7 @@ class LayoutEngine:
         c.eos, c.pad = d.eos_token_id, d.pad_token_id
         c.max_batch, c.s_max = max_batch, self.s_max
         c.max_rows, c.max_prefill_tokens = int(max_rows), int(max_prefill_tokens)
+        c.special_tokens, c.skew_scaler = d.special_token_count, d.skew_scaler
         self._wt = pack_layout_weights(cfg, sd_enc, sd_dec, dtype, self.device)     # keeps the device tensors alive
         arr = (ctypes.c_void_p * len(self._wt))(*[t.data_ptr() for t in self._wt])
         self._h = ctypes.c_void_p()
@@ -296,6 +298,54 @@ class LayoutEngine:
                                              _lib.stream_ptr()),
                    "sb_layout_decode")
         return hist["tok"], hist["bbox"], list(hist["heads"]), hist["done"]
+
+    def run_pages(self, enc: torch.Tensor, page_wh, n_steps: int):
+        """LayoutPredictor's decode loop (surya/layout/__init__.py:106-183) on the device through sb_layout_decode_pages: the
+        greedy pass of run_loop from the bos prompt, plus the header/footer relabelling of rows whose PageHeader / PageFooter box
+        lies away from the edges of their image (page_wh: (w, h) per row, the size the row was preprocessed from) and the stop
+        once every row has produced eos / pad.  Returns (tok [n, B, 7], bbox [n, B, 6], class logits [n, B, label_count] with the
+        relabelled logit zeroed, done [n, B] = this step's done flag) for the n <= n_steps steps that ran; views of buffers the
+        next call overwrites."""
+        if self.kind != "layout":
+            raise _lib.SuryaB200Error("run_pages needs a layout engine: page sizes drive LayoutPredictor's header/footer rule")
+        B = int(enc.shape[0])
+        wh = torch.as_tensor(page_wh, dtype=torch.int32).reshape(-1, 2) if not torch.is_tensor(page_wh) else page_wh
+        if tuple(wh.shape) != (B, 2):
+            raise _lib.SuryaB200Error(f"page_wh must be [{B}, 2] (w, h per row), got {tuple(wh.shape)}")
+        if n_steps < 1 or n_steps > self.s_max:
+            raise _lib.SuryaB200Error(f"{n_steps} steps need 1 <= n_steps <= s_max {self.s_max}")
+        if B < 1 or B > self.max_batch:
+            raise _lib.SuryaB200Error(f"batch {B} outside 1..max_batch {self.max_batch}")
+        enc_c = self._enc(enc)
+        hist = self._history("_phist", B, n_steps)
+        if "wh" not in hist:          # persistent: the step graphs read the page sizes through this pointer
+            hist["wh"] = torch.zeros((B, 2), dtype=torch.int32, device=self.device)
+            hist["bos"] = torch.full((B, 1, 7), self.cfg.decoder.bos_token_id, dtype=torch.int64, device=self.device)
+        hist["wh"].copy_(wh.to(torch.int32), non_blocking=False)
+        self._step_kv = False
+        n_run = ctypes.c_int(0)
+        _lib.check(self.lib.sb_layout_decode_pages(self._h, _lib.ptr(enc_c), ctypes.c_int(B), _lib.ptr(hist["bos"]), ctypes.c_int(1),
+                                                   _lib.ptr(hist["wh"]), ctypes.c_int(n_steps), _lib.ptr(hist["tok"]),
+                                                   _lib.ptr(hist["bbox"]), _lib.ptr(hist["heads"][0]), _lib.ptr(hist["done"]),
+                                                   ctypes.byref(n_run), _lib.stream_ptr()),
+                   "sb_layout_decode_pages")
+        n = n_run.value
+        return hist["tok"][:n], hist["bbox"][:n], hist["heads"][0][:n], hist["done"][:n]
+
+    def preprocess(self, pages_dev: torch.Tensor, jobs: torch.Tensor, tap_idx: torch.Tensor, tap_w: torch.Tensor,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """sb_layout_preprocess: uint8 pages packed in pages_dev (device), one job per output image (see layout_pages.plan_jobs)
+        -> NCHW pixel values [n_jobs, 3, H, W] in the engine dtype at the encoder size."""
+        H, W = self.cfg.encoder.image_size
+        n = int(jobs.shape[0])
+        if out is None:
+            out = torch.empty((n, 3, H, W), dtype=self.dtype, device=self.device)
+        if pages_dev.dtype != torch.uint8 or not pages_dev.is_cuda:
+            raise _lib.SuryaB200Error("pages must be a uint8 device buffer")
+        _lib.check(self.lib.sb_layout_preprocess(ctypes.c_int(ops.dt_code(self.dtype)), _lib.ptr(pages_dev), _lib.ptr(jobs),
+                                                 ctypes.c_int(n), _lib.ptr(tap_idx), _lib.ptr(tap_w), ctypes.c_int(H), ctypes.c_int(W),
+                                                 _lib.ptr(out), _lib.stream_ptr()), "sb_layout_preprocess")
+        return out
 
     # ---------------------------------------------------------------------------------------------- held cross K/V
     def cross_kv(self, enc: torch.Tensor):

@@ -45,6 +45,25 @@ def _bbox(poly):
     return [min(xs), min(ys), max(xs), max(ys)]
 
 
+def clean_keep(polys: Sequence, bbs: Sequence) -> List[int]:
+    """clean_boxes (surya/common/util.py:9-36): indices of the polygons kept, in order.  A polygon goes when its bbox is flat, or
+    when it lies inside the bbox of another polygon that differs from it both as a polygon and as a bbox."""
+    keep = []
+    for i, (p, bb) in enumerate(zip(polys, bbs)):
+        if bb[0] == bb[2] or bb[1] == bb[3]:
+            continue
+        contained = False
+        for q, ob in zip(polys, bbs):
+            if q == p or bb == ob:
+                continue
+            if bb[0] >= ob[0] and bb[1] >= ob[1] and bb[2] <= ob[2] and bb[3] <= ob[3]:
+                contained = True
+                break
+        if not contained:
+            keep.append(i)
+    return keep
+
+
 def page_polygons(boxes: Sequence[np.ndarray], confidences: Sequence[float], image_size: Tuple[int, int],
                   processor_size: Tuple[int, int]) -> Tuple[List[List[List[int]]], List[float]]:
     """get_and_clean_boxes + the vertical expansion of parallel_get_boxes (surya/detection/heatmap.py:125-175) on plain lists:
@@ -59,21 +78,8 @@ def page_polygons(boxes: Sequence[np.ndarray], confidences: Sequence[float], ima
         poly = [[max(min(x, iw), 0), max(min(y, ih), 0)] for x, y in poly]
         polys.append(poly)
     bbs = [_bbox(p) for p in polys]
-    keep = []
-    for i, (p, bb) in enumerate(zip(polys, bbs)):
-        if bb[0] == bb[2] or bb[1] == bb[3]:
-            continue
-        contained = False
-        for j, (q, ob) in enumerate(zip(polys, bbs)):
-            if q == p or bb == ob:
-                continue
-            if bb[0] >= ob[0] and bb[1] >= ob[1] and bb[2] <= ob[2] and bb[3] <= ob[3]:
-                contained = True
-                break
-        if not contained:
-            keep.append(i)
     out, conf = [], []
-    for i in keep:
+    for i in clean_keep(polys, bbs):
         p, bb = polys[i], bbs[i]
         w, h = bb[2] - bb[0], bb[3] - bb[1]
         if h < 3 * w:
