@@ -504,9 +504,13 @@ int sb_layout_decode_pages(sb_layout_engine* e, const void* enc, int batch, cons
  * cv2.resize(INTER_CUBIC, since the processor's resample 2 is cv2's INTER_CUBIC) of a uint8 RGB rectangle to out_w x out_h,
  * then x * (1/255) (double -> float), (x - 0.5) / 0.5 in float and the cast to `dtype` (fp16 / bf16), NCHW into out.
  * pages: uint8 HWC images packed in one buffer.  jobs int64 [n_jobs, 8]: byte offset of the page, page width (row pitch in
- * pixels), x0, y0 of the source rectangle, x and y tap-table rows, output row, 0.  Tap tables [rows, 4]: tap_idx int32 = source
- * column / row relative to the rectangle (already clamped to it), tap_w float32 = cubic weight; a table for an axis of n
- * source pixels scaled to m has m rows (surya_b200/layout_pages.py builds and caches them). */
+ * pixels), x0, y0 of the source rectangle, x and y tap-table rows, output row, page height.  Tap tables [rows, 4]: tap_idx int32 =
+ * source column / row relative to the rectangle (already clamped to it), tap_w float32 = cubic weight; a table for an axis of n
+ * source pixels scaled to m has m rows (surya_b200/layout_pages.py builds and caches them).
+ * Page height 0: the rectangle lies inside the page and every tap reads it.  Page height > 0 (a bounded job): a tap whose page
+ * coordinate (x0 + column, y0 + row) lies outside [0, page width) x [0, page height) reads 0 without touching memory, as PIL's
+ * Image.crop fills a crop box that extends past the page; x0 / y0 may then be negative and the rectangle may extend past the
+ * page.  The table_rec page flow (surya_b200/table_pages.py) crops its expanded table boxes this way. */
 int sb_layout_preprocess(int dtype, const unsigned char* pages, const long long* jobs, int n_jobs, const int* tap_idx,
                          const float* tap_w, int out_h, int out_w, void* out, void* stream);
 /* table_rec two-pass flow (TableRecPredictor.batch_table_recognition, surya/table_rec/__init__.py:134-236).

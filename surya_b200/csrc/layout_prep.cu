@@ -8,8 +8,11 @@
 //   astype(float64) * (1/255) -> float32, normalize(mean 0.5, std 0.5) in float32, then the predictor's cast to the model dtype
 //   (surya/layout/__init__.py:78-81; table_rec uses the same processor, surya/table_rec/processor.py:19-21).
 // A job reads a source rectangle (x0, y0, w, h) of a resident page, so ImageSlicer's crops (surya/layout/slicer.py:48-66) need no
-// copy.  The cubic taps (index relative to the rectangle, clamped to it = border replicate, and Keys weights with A = -0.75 from a
-// double-precision coordinate) are computed on the host per (source extent, destination extent) by surya_b200/layout_pages.py.
+// copy.  A job that gives the page height is bounded: taps outside the page read 0, as PIL's Image.crop fills a crop box that
+// extends past the page with black before the table processor's resize (surya/scripts/table_recognition.py:63-70), so the
+// expanded table boxes also need no copy.  The cubic taps (index relative to the rectangle, clamped to it = border replicate,
+// and Keys weights with A = -0.75 from a double-precision coordinate) are computed on the host per (source extent, destination
+// extent) by surya_b200/layout_pages.py.
 // Arithmetic (the model of OpenCV's uint8 cubic resize that oracle/layout_pages_oracle.py restates and pins to cv2): four
 // horizontal sums, each float32 tap by tap, then the vertical float32 sum, round half to even, clamp to 0..255.
 #include "ops.cuh"
@@ -22,7 +25,7 @@ namespace sb {
 namespace {
 
 constexpr int LP_TX = 32, LP_TY = 8;
-enum { LJ_SRC_OFF = 0, LJ_PITCH, LJ_X0, LJ_Y0, LJ_XTAB, LJ_YTAB, LJ_OUT, LJ_STRIDE = 8 };
+enum { LJ_SRC_OFF = 0, LJ_PITCH, LJ_X0, LJ_Y0, LJ_XTAB, LJ_YTAB, LJ_OUT, LJ_PAGE_H, LJ_STRIDE = 8 };
 
 template <typename T> __device__ __forceinline__ T to_dt(float v);
 template <> __device__ __forceinline__ __half to_dt<__half>(float v) { return __float2half_rn(v); }
@@ -57,18 +60,23 @@ __global__ void __launch_bounds__(LP_TX * LP_TY) layout_preprocess_kernel(const 
   const int x = x0 + threadIdx.x, y = y0 + threadIdx.y;
   if (x >= W || y >= H) return;
   const unsigned char* src = pages + j[LJ_SRC_OFF];
-  const size_t pitch = static_cast<size_t>(j[LJ_PITCH]) * 3;
+  const int page_w = static_cast<int>(j[LJ_PITCH]), page_h = static_cast<int>(j[LJ_PAGE_H]);
+  const size_t pitch = static_cast<size_t>(page_w) * 3;
   float acc[3] = {0.f, 0.f, 0.f};
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
-    const unsigned char* row = src + static_cast<size_t>(syi[threadIdx.y][r]) * pitch;
+    const int sy = syi[threadIdx.y][r];
+    const bool row_in = page_h == 0 || (sy >= 0 && sy < page_h);
+    const unsigned char* row = src + static_cast<ptrdiff_t>(sy) * static_cast<ptrdiff_t>(pitch);
     float hs[3] = {0.f, 0.f, 0.f};
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
-      const unsigned char* px = row + sxi[threadIdx.x][t] * 3;
+      const int sx = sxi[threadIdx.x][t];
+      const bool in = row_in && (page_h == 0 || (sx >= 0 && sx < page_w));   // outside a bounded job's page: PIL's 0 fill
+      const unsigned char* px = row + sx * 3;
       const float w = sxw[threadIdx.x][t];
 #pragma unroll
-      for (int c = 0; c < 3; ++c) hs[c] = __fadd_rn(hs[c], __fmul_rn(static_cast<float>(px[c]), w));
+      for (int c = 0; c < 3; ++c) hs[c] = __fadd_rn(hs[c], __fmul_rn(in ? static_cast<float>(px[c]) : 0.f, w));
     }
     const float w = syw[threadIdx.y][r];
 #pragma unroll

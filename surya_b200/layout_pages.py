@@ -11,7 +11,7 @@ from uint8 pages to per-page results.
                                       (:140-216), then ImageSlicer.join / merge_results (slicer.py:68-140)
 
 The results are plain dataclasses with the fields of the reference's LayoutResult / LayoutBox (surya/layout/schema.py) and the
-PolygonBox methods the slice join uses (surya/common/polygon.py).  No import of the reference or of oracle/.
+PolygonBox methods the slice join uses (surya/common/polygon.py, restated once in surya_b200/polygon.py).  No import of the reference or of oracle/.
 """
 from __future__ import annotations
 
@@ -26,6 +26,7 @@ import torch
 
 from ._lib import SuryaB200Error
 from .pipeline import clean_keep
+from .polygon import PolygonMethods
 
 SLICE_MIN = (1500, 1500)          # settings.LAYOUT_SLICE_MIN (width, height)
 SLICE_SIZE = (1200, 1200)         # settings.LAYOUT_SLICE_SIZE (width, height)
@@ -41,62 +42,12 @@ JOB_LEN = 8                       # int64 per job of sb_layout_preprocess
 
 # ------------------------------------------------------------------------------------------------ results
 @dataclass
-class LayoutBox:
+class LayoutBox(PolygonMethods):
     polygon: List[List[float]]
     label: str
     position: int
     top_k: Optional[Dict[str, float]] = None
     confidence: Optional[float] = None
-
-    @property
-    def bbox(self) -> List[float]:
-        xs = [p[0] for p in self.polygon]
-        ys = [p[1] for p in self.polygon]
-        return [min(xs), min(ys), max(xs), max(ys)]
-
-    @property
-    def width(self):
-        b = self.bbox
-        return b[2] - b[0]
-
-    @property
-    def height(self):
-        b = self.bbox
-        return b[3] - b[1]
-
-    @property
-    def area(self):
-        return self.width * self.height
-
-    def shift(self, x_shift=None, y_shift=None):
-        if x_shift is not None:
-            for p in self.polygon:
-                p[0] += x_shift
-        if y_shift is not None:
-            for p in self.polygon:
-                p[1] += y_shift
-
-    def merge(self, other: "LayoutBox"):
-        a, b = self.bbox, other.bbox
-        x1, y1, x2, y2 = min(a[0], b[0]), min(a[1], b[1]), max(a[2], b[2]), max(a[3], b[3])
-        self.polygon = [[x1, y1], [x2, y1], [x2, y2], [x1, y2]]
-
-    def x_overlap(self, other: "LayoutBox", x_margin=0):
-        a, b = self.bbox, other.bbox
-        return max(0, min(a[2] + x_margin, b[2] + x_margin) - max(a[0] - x_margin, b[0] - x_margin))
-
-    def y_overlap(self, other: "LayoutBox", y_margin=0):
-        a, b = self.bbox, other.bbox
-        return max(0, min(a[3] + y_margin, b[3] + y_margin) - max(a[1] - y_margin, b[1] - y_margin))
-
-    def intersection_pct(self, other: "LayoutBox", x_margin=0, y_margin=0):
-        if self.area == 0:
-            return 0
-        if x_margin:
-            x_margin = int(min(self.width, other.width) * x_margin)
-        if y_margin:
-            y_margin = int(min(self.height, other.height) * y_margin)
-        return self.x_overlap(other, x_margin) * self.y_overlap(other, y_margin) / self.area
 
 
 @dataclass
@@ -167,9 +118,12 @@ def cubic_axis(src: int, dst: int) -> Tuple[np.ndarray, np.ndarray]:
     return idx, w
 
 
-def plan_jobs(rects: Sequence[Tuple[int, int, int, int]], page_off: Sequence[int], page_w: Sequence[int], out_hw: Tuple[int, int]):
+def plan_jobs(rects: Sequence[Tuple[int, int, int, int]], page_off: Sequence[int], page_w: Sequence[int], out_hw: Tuple[int, int],
+              page_h: Optional[Sequence[int]] = None):
     """Job table and tap tables of sb_layout_preprocess.  rects[i] = (x0, y0, w, h) of the source rectangle of output i in the
-    page that starts at byte page_off[i] of the packed pages and is page_w[i] pixels wide.  Returns (jobs int64 [n, 8],
+    page that starts at byte page_off[i] of the packed pages and is page_w[i] pixels wide.  page_h (optional) gives page
+    heights: a job with a non-zero height is bounded, its taps outside the page read 0 (PIL's crop fill), and its rectangle may
+    extend past the page; without it every job has height 0 and must lie inside its page.  Returns (jobs int64 [n, 8],
     tap_idx int32 [rows, 4], tap_w float32 [rows, 4]) as CPU tensors; each (extent, out size) table appears once."""
     H, W = out_hw
     tables: Dict[Tuple[int, int], int] = {}
@@ -190,6 +144,8 @@ def plan_jobs(rects: Sequence[Tuple[int, int, int, int]], page_off: Sequence[int
     jobs = np.zeros((len(rects), JOB_LEN), np.int64)
     for n, (x0, y0, w, h) in enumerate(rects):
         jobs[n, :7] = (page_off[n], page_w[n], x0, y0, table(w, W), table(h, H), n)
+        if page_h is not None:
+            jobs[n, 7] = page_h[n]
     return (torch.from_numpy(jobs), torch.from_numpy(np.concatenate(idx_parts)), torch.from_numpy(np.concatenate(w_parts)))
 
 

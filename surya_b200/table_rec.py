@@ -4,8 +4,9 @@
   * TableRecRunner      per image batch: encoder once, cross K/V held once per table (LayoutEngine.cross_kv), the row/column
                         pass, the row queries / columns / cell prompts on the host, then the cell pass of every predicted row
                         against its table's held K/V (LayoutEngine.decode_rows: batched prompt prefill, early exit).  Returns
-                        the arguments the reference hands to decode_batch_predictions (:233), so a caller finishes with the
-                        reference's own geometry: predictor.decode_batch_predictions(*batch, LabelShaper()).
+                        the arguments the reference hands to decode_batch_predictions (:233); run_batch is one image batch.
+  * table_results       decode_batch_predictions (:239-387): the geometry that turns them into TableResults (TableCell /
+                        TableRow / TableCol with the reference schema's fields, to_dict() = model_dump()).
   * query_label / box_polygon / prompt builders: the processor's and shaper's host arithmetic (processor.py:29-82,
                         shaper.py:12-52, 83-142), float64 like the reference, truncated to int64 like torch.tensor(.., long).
 
@@ -14,13 +15,18 @@ of the reference and none of oracle/.
 """
 from __future__ import annotations
 
+import copy
+import itertools
 import math
+import time
+from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import _lib
+from .polygon import PolygonMethods
 
 BOX_DIM = 1024
 CATEGORY_TABLE, CATEGORY_ROW, CATEGORY_COLUMN = 4, 1, 2       # surya/table_rec/model/config.py ID_TO_CATEGORY
@@ -120,11 +126,13 @@ class TableRecRunner:
         self.engine, self.batch_size, self.max_boxes = engine, int(batch_size), int(max_boxes)
         self.cfg = engine.cfg.decoder
         self.trace: Optional[list] = None     # set to a list to keep every pass's inputs and step histories (host copies)
+        self.steps_run: List[int] = []        # decode steps of every pass, in order
 
     def _decode(self, row_table: List[int], prompt: torch.Tensor) -> List[List[Dict]]:
         n_steps = step_budget(self.max_boxes, prompt.shape[1])
         tok, bbox, heads, done = self.engine.decode_rows(row_table, prompt, n_steps)
         tok, bbox, done = tok.cpu(), bbox.cpu(), done.cpu()
+        self.steps_run.append(int(tok.shape[0]))
         if self.trace is not None:
             self.trace.append({"row_table": list(row_table), "prompt": prompt.cpu(), "n_steps": n_steps, "tok": tok, "bbox": bbox,
                                "heads": [h.cpu() for h in heads], "done": done})
@@ -135,29 +143,217 @@ class TableRecRunner:
         Returns one (rowcol_predictions, cell_predictions, idx_map, orig_sizes) per image batch of batch_size images."""
         if pixel_values.shape[0] != len(image_sizes):
             raise _lib.SuryaB200Error(f"{pixel_values.shape[0]} images but {len(image_sizes)} sizes")
+        return [self.run_batch(pixel_values[i:i + self.batch_size], image_sizes[i:i + self.batch_size])
+                for i in range(0, len(image_sizes), self.batch_size)]
+
+    def run_batch(self, pixel_values: torch.Tensor, image_sizes: Sequence[Tuple[int, int]], timing: Optional[Dict[str, float]] = None):
+        """One image batch (at most batch_size images): encoder, row/column pass, cell pass.  Returns (rowcol_predictions,
+        cell_predictions, idx_map, orig_sizes).  timing (optional): seconds added to its "encoder" and "passes" entries, with a
+        device synchronise after each phase."""
         eng, cfg = self.engine, self.cfg
-        out = []
-        for i in range(0, len(image_sizes), self.batch_size):
-            sizes = [tuple(int(v) for v in s) for s in image_sizes[i:i + self.batch_size]]
-            n = len(sizes)
-            enc = eng.encode(pixel_values[i:i + n])
-            eng.cross_kv(enc)
-            if self.trace is not None:
-                self.trace.append({"enc": enc.float().cpu()})
-            rowcol = self._decode(list(range(n)), table_query_prompt(sizes, cfg))
-            row_items, columns, idx_map = [], [], []
-            for j, preds in enumerate(rowcol):
-                for p in preds:
-                    item = {"polygon": box_polygon(p["bbox"]), "category": p["category"], "is_header": int(p["is_header"] == 1)}
-                    if p["category"] == CATEGORY_ROW:
-                        row_items.append(item)
-                        idx_map.append(j)
-                    elif p["category"] == CATEGORY_COLUMN:
-                        columns.append(item)
-            cells: List[List[Dict]] = []
-            if row_items:
-                prompts = cell_prompts(row_items, columns, cfg)
-                for r0 in range(0, len(row_items), eng.max_rows):
-                    cells.extend(self._decode(idx_map[r0:r0 + eng.max_rows], prompts[r0:r0 + eng.max_rows]))
-            out.append((rowcol, cells, idx_map, sizes))
-        return out
+        sizes = [tuple(int(v) for v in s) for s in image_sizes]
+        n = len(sizes)
+        if n < 1 or n > self.batch_size or pixel_values.shape[0] != n:
+            raise _lib.SuryaB200Error(f"a batch of {pixel_values.shape[0]} images with {n} sizes (batch_size {self.batch_size})")
+        t0 = time.perf_counter()
+        enc = eng.encode(pixel_values)
+        eng.cross_kv(enc)
+        if timing is not None:
+            _sync(eng)
+            t1 = time.perf_counter()
+            timing["encoder"] = timing.get("encoder", 0.0) + t1 - t0
+            t0 = t1
+        if self.trace is not None:
+            self.trace.append({"enc": enc.float().cpu()})
+        rowcol = self._decode(list(range(n)), table_query_prompt(sizes, cfg))
+        row_items, columns, idx_map = [], [], []
+        for j, preds in enumerate(rowcol):
+            for p in preds:
+                item = {"polygon": box_polygon(p["bbox"]), "category": p["category"], "is_header": int(p["is_header"] == 1)}
+                if p["category"] == CATEGORY_ROW:
+                    row_items.append(item)
+                    idx_map.append(j)
+                elif p["category"] == CATEGORY_COLUMN:
+                    columns.append(item)
+        cells: List[List[Dict]] = []
+        if row_items:
+            prompts = cell_prompts(row_items, columns, cfg)
+            for r0 in range(0, len(row_items), eng.max_rows):
+                cells.extend(self._decode(idx_map[r0:r0 + eng.max_rows], prompts[r0:r0 + eng.max_rows]))
+        if timing is not None:
+            timing["passes"] = timing.get("passes", 0.0) + time.perf_counter() - t0
+        return rowcol, cells, idx_map, sizes
+
+
+def _sync(engine):
+    if torch.device(engine.device).type == "cuda":
+        torch.cuda.synchronize(engine.device)
+
+
+# ------------------------------------------------------------------------------------------------ geometry
+MERGE_UP, MERGE_DOWN, MERGE_BOTH = 1, 2, 3                   # surya/table_rec/model/config.py MERGE_KEYS
+MERGE_VALUES = (MERGE_UP, MERGE_DOWN, MERGE_BOTH)
+
+
+def _float_polygon(polygon) -> List[List[float]]:
+    """PolygonBox's validator: a new list of float corners."""
+    return [[float(x), float(y)] for x, y in polygon]
+
+
+class _Polygon(PolygonMethods):
+    """A bare PolygonBox."""
+
+    def __init__(self, polygon):
+        self.polygon = _float_polygon(polygon)
+
+
+@dataclass
+class TableCell(PolygonMethods):
+    """surya/table_rec/schema.py TableCell."""
+    polygon: List[List[float]]
+    row_id: int
+    colspan: int
+    within_row_id: int
+    cell_id: int
+    is_header: bool
+    rowspan: Optional[int] = None
+    merge_up: bool = False
+    merge_down: bool = False
+    col_id: Optional[int] = None
+    confidence: Optional[float] = None
+    text_lines: Optional[List[dict]] = None
+
+    def __post_init__(self):
+        self.polygon = _float_polygon(self.polygon)
+
+    def to_dict(self) -> dict:
+        return {"polygon": [list(p) for p in self.polygon], "confidence": self.confidence, "row_id": self.row_id,
+                "colspan": self.colspan, "within_row_id": self.within_row_id, "cell_id": self.cell_id, "is_header": self.is_header,
+                "rowspan": self.rowspan, "merge_up": self.merge_up, "merge_down": self.merge_down, "col_id": self.col_id,
+                "text_lines": self.text_lines, "bbox": self.bbox}
+
+
+@dataclass
+class TableRow(PolygonMethods):
+    """surya/table_rec/schema.py TableRow."""
+    polygon: List[List[float]]
+    row_id: int
+    is_header: bool
+    confidence: Optional[float] = None
+
+    def __post_init__(self):
+        self.polygon = _float_polygon(self.polygon)
+
+    def to_dict(self) -> dict:
+        return {"polygon": [list(p) for p in self.polygon], "confidence": self.confidence, "row_id": self.row_id,
+                "is_header": self.is_header, "bbox": self.bbox}
+
+
+@dataclass
+class TableCol(PolygonMethods):
+    """surya/table_rec/schema.py TableCol."""
+    polygon: List[List[float]]
+    col_id: int
+    is_header: bool
+    confidence: Optional[float] = None
+
+    def __post_init__(self):
+        self.polygon = _float_polygon(self.polygon)
+
+    def to_dict(self) -> dict:
+        return {"polygon": [list(p) for p in self.polygon], "confidence": self.confidence, "col_id": self.col_id,
+                "is_header": self.is_header, "bbox": self.bbox}
+
+
+@dataclass
+class TableResult:
+    """surya/table_rec/schema.py TableResult; to_dict() is the reference's model_dump()."""
+    cells: List[TableCell]
+    unmerged_cells: List[TableCell]
+    rows: List[TableRow]
+    cols: List[TableCol]
+    image_bbox: List[float]
+
+    def to_dict(self) -> dict:
+        return {"cells": [c.to_dict() for c in self.cells], "unmerged_cells": [c.to_dict() for c in self.unmerged_cells],
+                "rows": [r.to_dict() for r in self.rows], "cols": [c.to_dict() for c in self.cols],
+                "image_bbox": [float(v) for v in self.image_bbox]}
+
+
+def _box_to_size(bbox, size) -> List[List[float]]:
+    return resize_polygon(box_polygon(bbox), (BOX_DIM, BOX_DIM), size)
+
+
+def table_results(rowcol, cells, idx_map, sizes) -> List[TableResult]:
+    """TableRecPredictor.decode_batch_predictions (surya/table_rec/__init__.py:239-387) for one image batch, from what
+    TableRecRunner.run_batch returns: columns and rows resized from BOX_DIM to the image, the spanning cells of every row, the
+    row x column cells, the merge of cells across rows on a copy of the row grid, and the de-duplication by cell_id."""
+    results = []
+    for j, (img_predictions, size) in enumerate(zip(rowcol, sizes)):
+        row_cells = [c for i, c in enumerate(cells) if idx_map[i] == j]
+        rows, unmerged, columns = [], [], []
+        cell_id = 0
+        row_preds = [p for p in img_predictions if p["category"] == CATEGORY_ROW]
+        col_preds = [p for p in img_predictions if p["category"] == CATEGORY_COLUMN]
+        for z, p in enumerate(col_preds):
+            columns.append(TableCol(polygon=_box_to_size(p["bbox"], size), col_id=z, is_header=p["is_header"] == 1))
+        for z, p in enumerate(row_preds):
+            row = TableRow(polygon=_box_to_size(p["bbox"], size), row_id=z, is_header=p["is_header"] == 1)
+            rows.append(row)
+            spanning = []
+            for l, sc in enumerate(row_cells[z]):
+                polygon = _box_to_size(sc["bbox"], size)
+                colspan = max(1, int(sc["colspan"]))
+                if colspan == 1 and sc["merges"] not in MERGE_VALUES:
+                    continue                                    # a single-column cell that does not merge
+                if _Polygon(polygon).height < row.height * .85:
+                    continue                                    # a spanning cell must cover most of the row
+                spanning.append(TableCell(polygon=polygon, row_id=z, rowspan=1, cell_id=cell_id, within_row_id=l, colspan=colspan,
+                                          merge_up=sc["merges"] in (MERGE_UP, MERGE_BOTH), merge_down=sc["merges"] in (MERGE_DOWN, MERGE_BOTH),
+                                          is_header=row.is_header or z == 0))
+                cell_id += 1
+            used = set()
+            skip = 0
+            for l, col in enumerate(columns):
+                if skip:
+                    skip -= 1
+                    continue
+                cell_polygon = row.intersection_polygon(col)
+                cell_box = _Polygon(cell_polygon)
+                added = False
+                for zz, sc in enumerate(spanning):
+                    col_width = sum(c.width for c in columns[l:l + sc.colspan])
+                    if cell_box.intersection_pct(sc) > .9:
+                        if sc.width > col_width * .85:
+                            added = True
+                            if zz not in used:
+                                used.add(zz)
+                                sc.col_id = l
+                                unmerged.append(sc)
+                                skip = sc.colspan - 1            # the columns the spanning cell covers
+                        else:
+                            used.add(zz)                         # too narrow for its colspan: never used
+                if not added:
+                    unmerged.append(TableCell(polygon=cell_polygon, row_id=z, rowspan=1, cell_id=cell_id, within_row_id=l, colspan=1,
+                                              merge_up=False, merge_down=False, col_id=l,
+                                              is_header=row.is_header or col.is_header or z == 0))
+                    cell_id += 1
+        grid = copy.deepcopy([[c for c in unmerged if c.row_id == r.row_id] for r in rows])
+        for z, grid_row in enumerate(grid[1:]):
+            prev = grid[z]
+            for l, c in enumerate(grid_row):
+                if l >= len(prev):
+                    continue
+                above = prev[l]
+                if above.merge_down and c.merge_up and above.col_id == c.col_id and above.colspan == c.colspan:
+                    above.merge(c)
+                    above.rowspan += c.rowspan
+                    grid_row[l] = above
+        merged, seen = [], set()
+        for c in itertools.chain.from_iterable(grid):
+            if c.cell_id not in seen:
+                seen.add(c.cell_id)
+                merged.append(c)
+        results.append(TableResult(cells=merged, unmerged_cells=unmerged, rows=rows, cols=columns,
+                                   image_bbox=[0, 0, size[0], size[1]]))
+    return results
